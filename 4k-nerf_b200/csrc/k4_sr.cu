@@ -1239,14 +1239,20 @@ static bool sr_no_tma() {
     return v == 1;
 }
 
+// Which convolution kernel runs a layer (the K4_CONV_KERNEL_* values of k4_testing_conv3x3).  SRK_AUTO is the decoder's
+// own choice, env switches included; a forced kernel either runs or the launch returns K4_ERR_UNSUPPORTED.
+enum SrKernel { SRK_AUTO = 0, SRK_WS_TMA = 1, SRK_WS_CPASYNC = 2, SRK_K64 = 3 };
+
 template <int N>
-int launch_conv_ws(ConvParams p, cudaStream_t s) {
+int launch_conv_ws(ConvParams p, cudaStream_t s, int sel, int* used) {
     using C = WsCfg<N>;
     if (int st = sr_set_smem(conv3x3_ws_kernel<N>, 3 + sr_bit_n(N), C::SMEM + SFTF_MAX)) return st;
     const int sms = sr_dev()->sms;
     alignas(64) CUtensorMap tm;
     memset(&tm, 0, sizeof(tm));
-    p.use_tma = (!p.upsample && !sr_no_tma() && sr_make_tmap(p, &tm)) ? 1 : 0;
+    const bool want_tma = (sel == SRK_AUTO) ? !sr_no_tma() : sel == SRK_WS_TMA;
+    p.use_tma = (!p.upsample && want_tma && sr_make_tmap(p, &tm)) ? 1 : 0;
+    if (sel == SRK_WS_TMA && !p.use_tma) return K4_ERR_UNSUPPORTED;
     const int tiles = ((p.W + WS_TX - 1) / WS_TX) * ((p.y_hi - p.y_lo + SR_TY - 1) / SR_TY);
     if (tiles <= 0) return K4_OK;
     size_t smem = C::SMEM;
@@ -1255,6 +1261,7 @@ int launch_conv_ws(ConvParams p, cudaStream_t s) {
         smem += sft_frag_layout(p.sft_n).total + (p.mode == SRM_TRUNK_SFT2 ? sft_frag_layout(64).total : 0);
     }
     K4_CUDA_TRY(sr_launch(conv3x3_ws_kernel<N>, (unsigned)(tiles < sms ? tiles : sms), WS_THREADS, smem, s, p, tm));
+    if (used) *used = p.use_tma ? SRK_WS_TMA : SRK_WS_CPASYNC;
     return K4_OK;
 }
 
@@ -1296,7 +1303,9 @@ static bool sr_use_k64() {
     return v == 1;
 }
 
-int run_conv(const SrConv& c, ConvParams p, cudaStream_t s, const __half* wk64_override = nullptr) {
+// sel: SrKernel; *used (if given) receives the kernel that ran.
+int run_conv(const SrConv& c, ConvParams p, cudaStream_t s, const __half* wk64_override = nullptr, int sel = SRK_AUTO,
+             int* used = nullptr) {
     const __half* wk64 = wk64_override ? wk64_override : ((p.ntaps == 0 || p.ntaps == 9) ? c.wk64 : nullptr);
     if (!p.wpack) p.wpack = c.wpack;
     p.bias = c.bias; p.cin = c.cin_pad;
@@ -1309,18 +1318,21 @@ int run_conv(const SrConv& c, ConvParams p, cudaStream_t s, const __half* wk64_o
     if (p.y_lo < 0) p.y_lo = 0;
     if (p.y_hi > p.H) p.y_hi = p.H;
     if (p.y_hi <= p.y_lo) return K4_OK;
-    if (sr_use_k64() && wk64 && p.cin == 64 && !p.upsample && (p.src_cstride % 8) == 0 && (p.src_c0 % 8) == 0 &&
-        (p.mode == SRM_STORE_F16 || p.mode == SRM_ADD_STORE_F16 || p.mode == SRM_OUT_NCHW)) {
-        const int st = (c.npad == 64) ? launch_conv_k64<64>(p, wk64, s) : (c.npad == 16) ? launch_conv_k64<16>(p, wk64, s) : K4_ERR_UNSUPPORTED;
-        if (st != K4_ERR_UNSUPPORTED) return st;
+    const bool k64_ok = wk64 && p.cin == 64 && !p.upsample && (p.src_cstride % 8) == 0 && (p.src_c0 % 8) == 0 &&
+                        (p.mode == SRM_STORE_F16 || p.mode == SRM_ADD_STORE_F16 || p.mode == SRM_OUT_NCHW);
+    if (sel == SRK_K64 || (sel == SRK_AUTO && sr_use_k64() && k64_ok)) {
+        const int st = !k64_ok ? K4_ERR_UNSUPPORTED : (c.npad == 64) ? launch_conv_k64<64>(p, wk64, s)
+                     : (c.npad == 16) ? launch_conv_k64<16>(p, wk64, s) : K4_ERR_UNSUPPORTED;
+        if (st == K4_OK && used) *used = SRK_K64;
+        if (st != K4_ERR_UNSUPPORTED || sel == SRK_K64) return st;
     }
-    if (c.npad == 64) return launch_conv_ws<64>(p, s);
-    if (c.npad == 32) return launch_conv_ws<32>(p, s);
-    return launch_conv_ws<16>(p, s);
+    if (c.npad == 64) return launch_conv_ws<64>(p, s, sel, used);
+    if (c.npad == 32) return launch_conv_ws<32>(p, s, sel, used);
+    return launch_conv_ws<16>(p, s, sel, used);
 }
 
 // nearest-x2 + conv as four sub-pixel convolutions over the source grid (p.H x p.W = SOURCE size, dst is 2H x 2W)
-int run_conv_up2x(const SrConv& c, ConvParams p, cudaStream_t s) {
+int run_conv_up2x(const SrConv& c, ConvParams p, cudaStream_t s, int sel = SRK_AUTO, int* used = nullptr) {
     for (int ph = 0; ph < 4; ++ph) {
         const int py = ph >> 1, px = ph & 1;
         ConvParams q = p;
@@ -1328,7 +1340,7 @@ int run_conv_up2x(const SrConv& c, ConvParams p, cudaStream_t s) {
         q.ntaps = 4;
         for (int t = 0; t < 4; ++t) { q.tap_dy[t] = (unsigned char)(py + (t >> 1)); q.tap_dx[t] = (unsigned char)(px + (t & 1)); }
         q.out_s = 2; q.out_oy = py; q.out_ox = px;
-        const int st = run_conv(c, q, s, c.wk64_phase[ph]);
+        const int st = run_conv(c, q, s, c.wk64_phase[ph], sel, used);
         if (st != K4_OK) return st;
     }
     return K4_OK;
@@ -1657,4 +1669,74 @@ extern "C" int k4_srnet_forward_roi_peers(const k4_srnet* n, const float* d_x, c
 extern "C" int k4_srnet_forward(const k4_srnet* n, const float* d_x, const float* d_cond, int32_t h, int32_t w,
                                 float* d_out, void* d_ws, size_t ws_bytes, k4_stream_t stream) {
     return k4_srnet_forward_roi(n, d_x, d_cond, h, w, 0, h, 0, w, d_out, (int64_t)16 * h * w, (int64_t)4 * w, d_ws, ws_bytes, stream);
+}
+
+// One decoder layer for the test suite: a throw-away k4_srnet holds the packs (make_conv & co., as k4_srnet_create
+// builds them), run_conv / run_conv_up2x run it with the requested kernel, k4_srnet_destroy frees it.
+extern "C" int k4_testing_conv3x3(const k4_conv_test_args* a, int32_t* kernel_used, k4_stream_t stream) {
+    if (kernel_used) *kernel_used = -1;
+    if (!a || !a->d_weight || !a->d_bias || !a->d_src) return K4_ERR_INVALID_ARG;
+    if (a->cout < 1 || a->cout > 64 || a->cin < 1 || a->cin > 192 || a->H < 1 || a->W < 1) return K4_ERR_INVALID_ARG;
+    if (a->mode < SRM_STORE_F16 || a->mode > SRM_TRUNK_SFT2) return K4_ERR_INVALID_ARG;
+    if (a->kernel < SRK_AUTO || a->kernel > SRK_K64) return K4_ERR_INVALID_ARG;
+    if (a->y_lo < 0 || a->y_lo >= a->y_hi || a->y_hi > a->H) return K4_ERR_INVALID_ARG;
+    const int cin_pad = (a->cin + 31) / 32 * 32, npad = a->cout <= 16 ? 16 : (a->cout <= 32 ? 32 : 64);
+    if (a->src_c0 < 0 || a->src_c0 % 8 || a->src_cstride % 8 || a->src_c0 + cin_pad > a->src_cstride) return K4_ERR_INVALID_ARG;
+    const int m = a->mode, oh = a->upsample2x ? 2 * a->H : a->H, ow = a->upsample2x ? 2 * a->W : a->W;
+    const bool sft = m >= SRM_STORE_F16_SFT;
+    if ((m == SRM_STORE_F16 || m == SRM_ADD_STORE_F16 || m == SRM_STORE_F16_SFT) &&
+        (!a->d_dst_h || a->dst_c0 < 0 || a->dst_c0 % 2 || a->dst_cstride % 2 || a->dst_c0 + npad > a->dst_cstride))
+        return K4_ERR_INVALID_ARG;
+    if ((m == SRM_TRUNK || m == SRM_ADD_STORE_F16) && !a->d_add_f) return K4_ERR_INVALID_ARG;
+    if ((m == SRM_TRUNK || m == SRM_STORE_F32F16 || m == SRM_TRUNK_SFT || m == SRM_TRUNK_SFT2) && !a->d_dst_f) return K4_ERR_INVALID_ARG;
+    if (m == SRM_OUT_NCHW && (!a->d_out_nchw || a->n_valid < 1 || a->n_valid > npad || a->out_plane_stride < 1 || a->out_row_stride < 1 ||
+                              a->crop_y0 < 0 || a->crop_y0 >= a->crop_y1 || a->crop_y1 > oh ||
+                              a->crop_x0 < 0 || a->crop_x0 >= a->crop_x1 || a->crop_x1 > ow))
+        return K4_ERR_INVALID_ARG;
+    if (sft) {
+        if (!a->d_cond16 || !a->h_sft || (m != SRM_STORE_F16_SFT && (!a->d_dst_h2 || a->dst2_c0 < 0 || a->dst2_c0 % 2 ||
+                                                                     a->dst2_cstride % 2 || a->dst2_c0 + npad > a->dst2_cstride)))
+            return K4_ERR_INVALID_ARG;
+        if (m == SRM_TRUNK_SFT2 && (!a->d_add_f2 || !a->h_sft2)) return K4_ERR_INVALID_ARG;
+        for (int i = 0; i < 8; ++i)
+            if (!a->h_sft[i] || (m == SRM_TRUNK_SFT2 && !a->h_sft2[i])) return K4_ERR_INVALID_ARG;
+    }
+    // built combinations only: SFT layers of 32 / 64 channels behind a direct convolution, the two-layer tail at 64
+    if (sft && (a->upsample2x || a->cout != npad || npad == 16 || (m == SRM_TRUNK_SFT2 && npad != 64))) return K4_ERR_UNSUPPORTED;
+    int st = k4_device_check();
+    if (st != K4_OK) return st;
+
+    cudaStream_t s = (cudaStream_t)stream;
+    k4_srnet* n = new (std::nothrow) k4_srnet();
+    if (!n) return K4_ERR_INVALID_ARG;
+    memset(n, 0, sizeof(*n));
+    SrConv& c = n->conv_first;
+    SrSft& f1 = n->sftbody;
+    SrSft& f2 = n->rrdb_sft[0];
+    st = make_conv(n, c, a->d_weight, a->d_bias, a->cout, a->cin, s);
+    if (!st && a->upsample2x) st = make_conv_phases(n, c, a->d_weight, a->cout, a->cin, s);
+    if (!st) st = make_conv_k64(n, c, a->d_weight, a->cout, a->cin, a->upsample2x != 0, s);
+    if (!st && sft) st = make_sft(n, f1, a->h_sft, a->cout, s);
+    if (!st && m == SRM_TRUNK_SFT2) st = make_sft(n, f2, a->h_sft2, 64, s);
+    int used = -1;
+    if (!st) {
+        ConvParams p{};
+        p.src = static_cast<const __half*>(a->d_src); p.src_cstride = a->src_cstride; p.src_c0 = a->src_c0;
+        p.H = a->H; p.W = a->W; p.y_lo = a->y_lo; p.y_hi = a->y_hi;
+        p.mode = m; p.lrelu = a->lrelu; p.scale = a->scale; p.scale2 = a->scale2;
+        p.dst_h = static_cast<__half*>(a->d_dst_h); p.dst_cstride = a->dst_cstride; p.dst_c0 = a->dst_c0;
+        p.dst_f = a->d_dst_f; p.dst_f2 = a->d_dst_f2; p.add_f = a->d_add_f; p.add_f2 = a->d_add_f2;
+        p.dst_h2 = static_cast<__half*>(a->d_dst_h2); p.dst2_cstride = a->dst2_cstride; p.dst2_c0 = a->dst2_c0;
+        p.out_nchw = a->d_out_nchw; p.n_valid = a->n_valid; p.out_ps = a->out_plane_stride; p.out_rs = a->out_row_stride;
+        p.crop_y0 = a->crop_y0; p.crop_y1 = a->crop_y1; p.crop_x0 = a->crop_x0; p.crop_x1 = a->crop_x1;
+        p.cond16 = static_cast<const __half*>(a->d_cond16);
+        if (sft) { p.sftw = f1.frag; p.sft_n = a->cout; }
+        if (m == SRM_TRUNK_SFT2) p.sftw2 = f2.frag;
+        st = a->upsample2x ? run_conv_up2x(c, p, s, a->kernel, &used) : run_conv(c, p, s, nullptr, a->kernel, &used);
+    }
+    const cudaError_t e = cudaStreamSynchronize(s);       // the packs are freed below
+    if (st == K4_OK && e != cudaSuccess) { k4_set_cuda_error(e, "k4_testing_conv3x3"); st = K4_ERR_CUDA; }
+    k4_srnet_destroy(n);
+    if (st == K4_OK && kernel_used) *kernel_used = used;
+    return st;
 }

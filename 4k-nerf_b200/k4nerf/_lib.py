@@ -60,6 +60,27 @@ class SrnetDesc(C.Structure):
     ]
 
 
+K4_CONV_KERNEL_AUTO, K4_CONV_KERNEL_WS_TMA, K4_CONV_KERNEL_WS_CPASYNC, K4_CONV_KERNEL_K64 = 0, 1, 2, 3
+
+
+class ConvTestArgs(C.Structure):
+    """k4_conv_test_args: one decoder convolution for the test suite (k4_testing_conv3x3)."""
+    _fields_ = [
+        ('d_weight', C.c_void_p), ('d_bias', C.c_void_p), ('cout', C.c_int32), ('cin', C.c_int32),
+        ('d_src', C.c_void_p), ('src_cstride', C.c_int32), ('src_c0', C.c_int32), ('H', C.c_int32), ('W', C.c_int32),
+        ('upsample2x', C.c_int32), ('mode', C.c_int32), ('lrelu', C.c_float), ('scale', C.c_float), ('scale2', C.c_float),
+        ('y_lo', C.c_int32), ('y_hi', C.c_int32),
+        ('d_dst_h', C.c_void_p), ('dst_cstride', C.c_int32), ('dst_c0', C.c_int32),
+        ('d_dst_f', C.c_void_p), ('d_dst_f2', C.c_void_p), ('d_add_f', C.c_void_p), ('d_add_f2', C.c_void_p),
+        ('d_dst_h2', C.c_void_p), ('dst2_cstride', C.c_int32), ('dst2_c0', C.c_int32),
+        ('d_out_nchw', C.c_void_p), ('n_valid', C.c_int32), ('reserved0', C.c_int32),
+        ('out_plane_stride', C.c_int64), ('out_row_stride', C.c_int64),
+        ('crop_y0', C.c_int32), ('crop_y1', C.c_int32), ('crop_x0', C.c_int32), ('crop_x1', C.c_int32),
+        ('d_cond16', C.c_void_p), ('h_sft', C.POINTER(C.c_void_p)), ('h_sft2', C.POINTER(C.c_void_p)),
+        ('kernel', C.c_int32), ('reserved1', C.c_int32),
+    ]
+
+
 EXPORTS = {
     'k4_abi_version': (C.c_int, []),
     'k4_status_string': (C.c_char_p, [C.c_int]),
@@ -118,6 +139,7 @@ EXPORTS = {
                                     C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'k4_make_rays': (C.c_int, [C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_int32,
                                C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'k4_testing_conv3x3': (C.c_int, [C.POINTER(ConvTestArgs), C.POINTER(C.c_int32), C.c_void_p]),
 }
 
 if not os.path.exists(LIB_PATH):

@@ -351,6 +351,71 @@ K4_API int k4_op_grid_sample(const float* d_grid, int32_t C, int32_t X, int32_t 
 K4_API int k4_op_grid_sample_backward(const float* d_grad_out, int32_t C, int32_t X, int32_t Y, int32_t Z, const float* h_xyz_min,
                                       const float* h_xyz_max, const float* d_xyz, int64_t M, float* d_grad_grid, k4_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Testing.  Entry points for the test suite, not for renderers: they replace no reference interface and may change
+ * with the kernels they expose.
+ *
+ * k4_testing_conv3x3: ONE VC-Decoder convolution layer, packed by the same weight packers k4_srnet_create uses and run
+ * by the same dispatcher as k4_srnet_forward, so that a test can compare a single layer with a reference.
+ *   d_weight [cout][cin][3][3], d_bias [cout] fp32; cout <= 64, cin <= 192.  Inputs are padded to cin_pad = 32 *
+ *   ceil(cin / 32) channels (the decoder's NHWC layouts); the layer computes npad = 16 | 32 | 64 output channels
+ *   (cout rounded up), the ones beyond cout with zero weights and bias.
+ *   d_src: fp16 NHWC, channels [src_c0, src_c0 + cin_pad) of src_cstride per pixel (both multiples of 8), H x W pixels.
+ *   upsample2x: "nearest x2, then conv" in its sub-pixel form; the output is 2H x 2W (modes 0-4 only).
+ *   Output rows [y_lo, y_hi) of the H x W iteration grid (the source grid when upsample2x), 0 <= y_lo < y_hi <= H.
+ *   mode (the epilogues of csrc/k4_sr.cu, pixels p of the output grid, fp32 per-pixel buffers have 64 channels):
+ *     0 dst_h[p][dst_c0 + c] = fp16(act(conv + b)), act = LeakyReLU(lrelu) if lrelu > 0
+ *     1 dst_f = (conv + b) * scale + add_f
+ *     2 dst_h = fp16((conv + b) + add_f)
+ *     3 dst_f = dst_f2 = conv + b                          (dst_f2 may be NULL)
+ *     4 d_out_nchw[c * out_plane_stride + (y - crop_y0) * out_row_stride + (x - crop_x0)] = conv + b for c < n_valid and
+ *       (y, x) inside [crop_y0, crop_y1) x [crop_x0, crop_x1)
+ *     5 dst_h = fp16(sft(act(conv + b)))                                            (cout 32 or 64)
+ *     6 t = (conv + b) * scale [+ add_f]; dst_f [, dst_f2] = t; dst_h2 = fp16(sft(t))           (cout 32 or 64)
+ *     7 t as in 6; u = sft(t) * scale2 + add_f2; dst_f = u; dst_h2 = fp16(sft2(u))               (cout 64)
+ *   sft(x) = x * (scale + 1) + shift of an SFT layer with condition d_cond16 (fp16 [H*W][32]); h_sft / h_sft2: HOST
+ *   arrays of the 8 device pointers of its 1x1 convolutions in k4_srnet_desc order (scale_conv0 w, b, scale_conv1 w, b,
+ *   shift_conv0 w, b, shift_conv1 w, b).
+ *   kernel: K4_CONV_KERNEL_AUTO picks what k4_srnet_forward would (environment switches included); any other value
+ *   forces that kernel, which runs or the call returns K4_ERR_UNSUPPORTED.  *kernel_used (may be NULL) receives the
+ *   kernel that ran.  Arguments are checked before any CUDA call (K4_ERR_INVALID_ARG).  The call synchronises `stream`.
+ */
+enum { K4_CONV_KERNEL_AUTO = 0,            /* the decoder's own choice                           */
+       K4_CONV_KERNEL_WS_TMA = 1,          /* conv3x3_ws_kernel, TMA producer                    */
+       K4_CONV_KERNEL_WS_CPASYNC = 2,      /* conv3x3_ws_kernel, cp.async producer               */
+       K4_CONV_KERNEL_K64 = 3 };           /* conv3x3_k64_kernel (cin_pad 64, npad 16 or 64)     */
+
+typedef struct k4_conv_test_args {
+    const float* d_weight;
+    const float* d_bias;
+    int32_t cout, cin;
+    const void* d_src;                     /* fp16 */
+    int32_t src_cstride, src_c0;
+    int32_t H, W;
+    int32_t upsample2x;
+    int32_t mode;
+    float lrelu, scale, scale2;
+    int32_t y_lo, y_hi;
+    void* d_dst_h;                         /* fp16 */
+    int32_t dst_cstride, dst_c0;
+    float* d_dst_f;
+    float* d_dst_f2;
+    const float* d_add_f;
+    const float* d_add_f2;
+    void* d_dst_h2;                        /* fp16 */
+    int32_t dst2_cstride, dst2_c0;
+    float* d_out_nchw;
+    int32_t n_valid, reserved0;
+    int64_t out_plane_stride, out_row_stride;
+    int32_t crop_y0, crop_y1, crop_x0, crop_x1;
+    const void* d_cond16;                  /* fp16 */
+    const float* const* h_sft;
+    const float* const* h_sft2;
+    int32_t kernel;
+    int32_t reserved1;
+} k4_conv_test_args;
+K4_API int k4_testing_conv3x3(const k4_conv_test_args* args, int32_t* kernel_used, k4_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
