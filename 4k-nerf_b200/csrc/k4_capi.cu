@@ -415,7 +415,7 @@ extern "C" int k4_scene_create(const k4_scene_desc* d, k4_stream_t stream, k4_sc
                 pack_tc_bias_kernel<<<1, 256, 0, s>>>(d->d_rgbnet_bias[2], blob + BL.off_b3, 3, 16);
                 pack_tc_ones_kernel<<<8, 256, 0, s>>>(blob + BL.off_ones);
                 K4_CTRY(cudaGetLastError());
-                v.tc_blob = blob; v.tc_kpad = kpad; v.tc_width = w; v.tc_cfg = c.id;
+                v.tc_blob = blob; v.tc_kpad = kpad; v.tc_width = w; v.tc_cfg = c.id; v.tc_colmap = d_colmap;
                 v.tc_exact = (c.C == v.C && c.vpe == v.viewpe && c.spe == v.spape && c.W == v.width) ? 1 : 0;
             }
         }
@@ -520,6 +520,115 @@ extern "C" int k4_render_rays_frames(const k4_scene* sc, const k4_render_args* a
                                      void* d_workspace, size_t workspace_bytes, k4_stream_t stream) {
     if (!dst) return K4_ERR_INVALID_ARG;
     return render_impl(sc, a, d_rays_o, d_rays_d, d_viewdirs, n_rays, out, dst, d_workspace, workspace_bytes, stream);
+}
+
+// ---- the rgbnet of one MLP mode on caller-supplied rows (test suite) ----
+// These kernels live here rather than in k4_march.cu so that the marcher's translation unit, and with it the code of
+// the __noinline__ mlp_fp32 / MmaWarpCtx::flush it calls, is unchanged by them.
+namespace {
+
+// F16 / F16X3: one warp per group of 32 rows, driven through MmaWarpCtx as k4_march_kernel drives it: push_row of the
+// group's rows (a full group flushes there), end_tile (flushes a partial group, hands back the per-lane accumulators).
+template <int MODE>
+__global__ void __launch_bounds__(K4_MARCH_THREADS)
+k4_test_rgbnet_mma_kernel(const __grid_constant__ K4Dev s, const float* __restrict__ xs, const float* __restrict__ diffs,
+                          const float* __restrict__ ws, const int* __restrict__ owners, long long n, float* __restrict__ racc) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    MmaWarpCtx<MODE> mma;
+    mma.init(s, smem_raw, warp, lane);
+    const long long n_groups = (n + 31) / 32;
+    for (long long g = (long long)blockIdx.x * K4_MARCH_WARPS + warp; g < n_groups; g += (long long)gridDim.x * K4_MARCH_WARPS) {
+        const long long r = g * 32 + lane;
+        const bool shade = r < n;
+        float x[64], d[3] = {0.f, 0.f, 0.f}, w = 0.f;
+        int o = 0;
+        if (shade) {
+            for (int k = 0; k < s.kpad[0]; ++k) x[k] = k < s.dim0 ? xs[r * s.dim0 + k] : 0.f;
+            if (diffs) { d[0] = diffs[3 * r]; d[1] = diffs[3 * r + 1]; d[2] = diffs[3 * r + 2]; }
+            w = ws[r];
+            o = owners[r] & 31;
+        }
+        mma.push_row(s, shade, w, x, diffs ? d : nullptr, o, lane);
+        float cr, cg, cb;
+        mma.end_tile(s, lane, cr, cg, cb);
+        racc[3 * (g * 32 + lane) + 0] = cr; racc[3 * (g * 32 + lane) + 1] = cg; racc[3 * (g * 32 + lane) + 2] = cb;
+    }
+}
+
+// FP32: thread (group g, owner j) walks the group's rows in order and accumulates the ones it owns, as k4_march_kernel
+// accumulates a ray's samples
+__global__ void k4_test_rgbnet_fp32_kernel(const __grid_constant__ K4Dev s, const float* __restrict__ xs, const float* __restrict__ diffs,
+                                           const float* __restrict__ ws, const int* __restrict__ owners, long long n,
+                                           float* __restrict__ racc) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long g = i >> 5;
+    const int j = (int)(i & 31);
+    if (g * 32 >= n) return;
+    float acc_r = 0.f, acc_g = 0.f, acc_b = 0.f;
+    for (long long r = g * 32; r < n && r < g * 32 + 32; ++r) {
+        if ((owners[r] & 31) != j) continue;
+        float rgb[3];
+        mlp_fp32(s, xs + r * s.dim0, rgb);
+        if (diffs) {
+            rgb[0] = __fadd_rn(rgb[0], diffs[3 * r]); rgb[1] = __fadd_rn(rgb[1], diffs[3 * r + 1]);
+            rgb[2] = __fadd_rn(rgb[2], diffs[3 * r + 2]);
+        }
+        rgb[0] = sigmoid_ref(rgb[0]); rgb[1] = sigmoid_ref(rgb[1]); rgb[2] = sigmoid_ref(rgb[2]);
+        const float w = ws[r];
+        acc_r = __fadd_rn(acc_r, __fmul_rn(w, rgb[0]));
+        acc_g = __fadd_rn(acc_g, __fmul_rn(w, rgb[1]));
+        acc_b = __fadd_rn(acc_b, __fmul_rn(w, rgb[2]));
+    }
+    racc[3 * i + 0] = acc_r; racc[3 * i + 1] = acc_g; racc[3 * i + 2] = acc_b;
+}
+
+template <int MODE>
+int launch_test_rgbnet_mma(const K4Dev& v, const k4_rgbnet_test_args* a, cudaStream_t st) {
+    auto kern = k4_test_rgbnet_mma_kernel<MODE>;
+    const size_t smem = MmaWarpCtx<MODE>::smem_bytes(v);
+    if (smem > 48 * 1024) K4_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const long long n_groups = (a->n + 31) / 32;
+    long long blocks = (n_groups + K4_MARCH_WARPS - 1) / K4_MARCH_WARPS;
+    if (blocks > 1024) blocks = 1024;
+    kern<<<(unsigned)blocks, K4_MARCH_THREADS, smem, st>>>(v, a->d_x, a->d_diffuse, a->d_w, a->d_owner, a->n, a->d_racc);
+    K4_CUDA_TRY(cudaGetLastError());
+    return K4_OK;
+}
+
+int testing_rgbnet_mma(const K4Dev& v, const k4_rgbnet_test_args* a, cudaStream_t st) {
+    if (a->mode == K4_MLP_F16) return launch_test_rgbnet_mma<K4_MLP_F16>(v, a, st);
+    if (a->mode == K4_MLP_F16X3) return launch_test_rgbnet_mma<K4_MLP_F16X3>(v, a, st);
+    if (a->mode != K4_MLP_FP32) return K4_ERR_UNSUPPORTED;
+    const long long threads = (a->n + 31) / 32 * 32;
+    k4_test_rgbnet_fp32_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, st>>>(v, a->d_x, a->d_diffuse, a->d_w, a->d_owner, a->n,
+                                                                                 a->d_racc);
+    K4_CUDA_TRY(cudaGetLastError());
+    return K4_OK;
+}
+
+}  // namespace
+
+extern "C" int k4_testing_rgbnet(const k4_scene* sc, const k4_rgbnet_test_args* a, int32_t* group_rows, k4_stream_t stream) {
+    if (group_rows) *group_rows = 0;
+    if (!sc || !a) return K4_ERR_INVALID_ARG;
+    if (a->mode < K4_MLP_FP32 || a->mode > K4_MLP_TCGEN05_WS) return K4_ERR_INVALID_ARG;
+    if (a->n < 1 || a->n > (1ll << 24)) return K4_ERR_INVALID_ARG;
+    if (!a->d_x || !a->d_w || !a->d_owner || !a->d_racc) return K4_ERR_INVALID_ARG;
+    const K4Dev& v = sc->dev;
+    const bool diffuse = v.kind == K4_KIND_DVGO && !v.direct;
+    if (diffuse != (a->d_diffuse != nullptr)) return K4_ERR_INVALID_ARG;
+    const bool wgmma = a->mode == K4_MLP_TCGEN05 || a->mode == K4_MLP_TCGEN05_WS;
+    if (v.depth == 0) return K4_ERR_UNSUPPORTED;
+    if (wgmma && !k4_ws_supported(v)) return K4_ERR_UNSUPPORTED;
+    if (a->mode == K4_MLP_F16 && !MmaWarpCtx<K4_MLP_F16>::supported(v)) return K4_ERR_UNSUPPORTED;
+    if (a->mode == K4_MLP_F16X3 && !MmaWarpCtx<K4_MLP_F16X3>::supported(v)) return K4_ERR_UNSUPPORTED;
+    cudaStream_t s = (cudaStream_t)stream;
+    int st = wgmma ? k4_testing_rgbnet_ws(sc, a, s) : testing_rgbnet_mma(v, a, s);
+    const cudaError_t e = cudaStreamSynchronize(s);
+    if (st == K4_OK && e != cudaSuccess) { k4_set_cuda_error(e, "k4_testing_rgbnet"); st = K4_ERR_CUDA; }
+    if (st == K4_OK && group_rows) *group_rows = wgmma ? 128 : 32;
+    return st;
 }
 
 // ---- device memory shared between the ranks of a node (CUDA IPC; one process per GPU) ----

@@ -47,6 +47,7 @@ struct K4Dev {
     // DirectContractedVoxGO (lib/dcvgo.py)
     float scene_center[3], scene_radius[3], bg_len, one_plus_bg;
     int world_len;
+    const int* tc_colmap;         // [dim0]: column of every model input in the tc_cfg entry's row layout (k4_testing_rgbnet)
 };
 
 // ---- wgmma operand blob (built by k4_scene_create, staged by one TMA bulk copy) -------------------
@@ -125,3 +126,5 @@ int k4_launch_march_tc(const k4_scene* sc, K4RenderParams rp, cudaStream_t st); 
 bool k4_tc_supported(const K4Dev& v);
 bool k4_ws_supported(const K4Dev& v);
 int k4_launch_march_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st);   // warp-specialised variant (same shapes)
+// k4_testing_rgbnet for the wgmma modes (arguments already checked; k4_capi.cu runs the other modes)
+int k4_testing_rgbnet_ws(const k4_scene* sc, const k4_rgbnet_test_args* a, cudaStream_t st);

@@ -330,9 +330,9 @@ int launch_variant(const k4_scene* sc, const K4RenderParams& rp, cudaStream_t st
 int k4_launch_march(const k4_scene* sc, const K4RenderParams& rp, int mlp_mode, cudaStream_t st) {
     if (sc->dev.kind == K4_KIND_DCVGO) {
         if (mlp_mode == K4_MLP_FP32 || sc->dev.depth == 0) return launch_variant<K4_KIND_DCVGO, K4_MLP_FP32>(sc, rp, st);
-        if (!MmaWarpCtx<K4_MLP_F16>::supported(sc->dev)) return K4_ERR_UNSUPPORTED;
-        if (mlp_mode == K4_MLP_F16) return launch_variant<K4_KIND_DCVGO, K4_MLP_F16>(sc, rp, st);
-        if (mlp_mode == K4_MLP_F16X3) return launch_variant<K4_KIND_DCVGO, K4_MLP_F16X3>(sc, rp, st);
+        if (mlp_mode == K4_MLP_F16 && MmaWarpCtx<K4_MLP_F16>::supported(sc->dev)) return launch_variant<K4_KIND_DCVGO, K4_MLP_F16>(sc, rp, st);
+        if (mlp_mode == K4_MLP_F16X3 && MmaWarpCtx<K4_MLP_F16X3>::supported(sc->dev))
+            return launch_variant<K4_KIND_DCVGO, K4_MLP_F16X3>(sc, rp, st);
         return K4_ERR_UNSUPPORTED;
     }
     const bool mpi = sc->dev.kind == K4_KIND_DMPIGO;
@@ -340,12 +340,11 @@ int k4_launch_march(const k4_scene* sc, const K4RenderParams& rp, int mlp_mode, 
         return mpi ? launch_variant<K4_KIND_DMPIGO, K4_MLP_FP32>(sc, rp, st)
                    : launch_variant<K4_KIND_DVGO, K4_MLP_FP32>(sc, rp, st);
     }
-    if (!MmaWarpCtx<K4_MLP_F16>::supported(sc->dev)) return K4_ERR_UNSUPPORTED;
-    if (mlp_mode == K4_MLP_F16) {
+    if (mlp_mode == K4_MLP_F16 && MmaWarpCtx<K4_MLP_F16>::supported(sc->dev)) {
         return mpi ? launch_variant<K4_KIND_DMPIGO, K4_MLP_F16>(sc, rp, st)
                    : launch_variant<K4_KIND_DVGO, K4_MLP_F16>(sc, rp, st);
     }
-    if (mlp_mode == K4_MLP_F16X3) {
+    if (mlp_mode == K4_MLP_F16X3 && MmaWarpCtx<K4_MLP_F16X3>::supported(sc->dev)) {
         return mpi ? launch_variant<K4_KIND_DMPIGO, K4_MLP_F16X3>(sc, rp, st)
                    : launch_variant<K4_KIND_DVGO, K4_MLP_F16X3>(sc, rp, st);
     }

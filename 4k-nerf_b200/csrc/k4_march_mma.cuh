@@ -127,8 +127,10 @@ struct MmaWarpCtx {
     int n_batches;
     int ks1;                      // k16 steps of layer 1
 
+    // The shape is built and this mode's shared memory fits a block (sm_90: 227 KB).  F16X3 holds two weight parts and
+    // two rings, which do not fit for width 128 with 49..64 inputs (kpad 64).
     __host__ __device__ static bool supported(const K4Dev& s) {
-        return s.depth == 3 && (s.width == 128 || s.width == 64) && s.dim0 <= 64 && s.dim0 > 0;
+        return s.depth == 3 && (s.width == 128 || s.width == 64) && s.dim0 <= 64 && s.dim0 > 0 && smem_bytes(s) <= 227 * 1024;
     }
 
     __host__ __device__ static int a_stride(const K4Dev& s) { return s.kpad[0] + 8; }
@@ -203,13 +205,10 @@ struct MmaWarpCtx {
     template <int KIND, typename CellT>
     __device__ void push(const K4Dev& s, bool shade, float w, const CellT& cell, const float cw[8],
                          const int cidx[8], const float* vemb, int n_vemb, int lane) {
-        const unsigned bal = __ballot_sync(0xffffffffu, shade);
-        if (bal == 0) return;
+        float k0v[32];
+        float x[64];
         if (shade) {
-            const int slot = (head + count + __popc(bal & ((1u << lane) - 1))) & (kRing - 1);
-            float k0v[32];
             interp_k0<8>(s, cw, cidx, k0v);
-            float x[64];
             int n = 0;
             for (int c = s.k0_view_off; c < s.C; ++c) x[n++] = k0v[c];
             if (KIND == K4_KIND_DMPIGO) {
@@ -219,6 +218,19 @@ struct MmaWarpCtx {
             for (int c = 0; c < n_vemb; ++c) x[n++] = vemb[c];
             const int kp = s.kpad[0];
             for (; n < kp; ++n) x[n] = 0.f;
+        }
+        push_row(s, shade, w, x, (KIND == K4_KIND_DVGO && !s.direct) ? k0v : nullptr, lane, lane);
+    }
+
+    // Append a row x[0 .. kpad[0]) (model-layout inputs, zero padded) owned by `owner` to the ring, with its diffuse
+    // logits diff[0..2] (nullptr: none); run the MLP when 32 rows are pending.  Called by all 32 lanes.
+    __device__ __forceinline__ void push_row(const K4Dev& s, bool shade, float w, const float* x, const float* diff,
+                                             int owner, int lane) {
+        const unsigned bal = __ballot_sync(0xffffffffu, shade);
+        if (bal == 0) return;
+        if (shade) {
+            const int slot = (head + count + __popc(bal & ((1u << lane) - 1))) & (kRing - 1);
+            const int kp = s.kpad[0];
             uint32_t* rh = reinterpret_cast<uint32_t*>(a_part[0] + (size_t)slot * astride * 2);
             uint32_t* rl = kX3 ? reinterpret_cast<uint32_t*>(a_part[1] + (size_t)slot * astride * 2) : nullptr;
             for (int j = 0; j < kp; j += 2) {
@@ -231,9 +243,9 @@ struct MmaWarpCtx {
                 }
             }
             qw[slot] = w;
-            qowner[slot] = (unsigned char)lane;
-            if (KIND == K4_KIND_DVGO && !s.direct) {
-                qdiff[slot * 3 + 0] = k0v[0]; qdiff[slot * 3 + 1] = k0v[1]; qdiff[slot * 3 + 2] = k0v[2];
+            qowner[slot] = (unsigned char)owner;
+            if (diff) {
+                qdiff[slot * 3 + 0] = diff[0]; qdiff[slot * 3 + 1] = diff[1]; qdiff[slot * 3 + 2] = diff[2];
             }
         }
         count += __popc(bal);

@@ -504,7 +504,86 @@ int launch_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st) {
     return K4_OK;
 }
 
+// k4_testing_rgbnet, wgmma modes: one CTA = one warpgroup = one batch of up to 128 caller rows.  The operand blob is staged
+// as the marchers stage it; row r goes to ring-tile row r through the scene's column map (pack2, other columns zero), its
+// weight / owner / diffuse logits to the queue, and mlp_batch_wgmma accumulates the colours into racc.
+template <class Cfg>
+__global__ void __launch_bounds__(TC_WG, 1)
+k4_test_rgbnet_ws_kernel(const __grid_constant__ K4Dev s, const float* __restrict__ xs, const float* __restrict__ diffs,
+                         const float* __restrict__ ws, const int* __restrict__ owners, long long n, float* __restrict__ racc_out) {
+    extern __shared__ __align__(1024) unsigned char smem[];
+    constexpr int W = Cfg::W, KPAD = Cfg::KPAD, KCH = Cfg::KCH;
+    unsigned char* blob = smem;
+    unsigned char* tile = smem + Cfg::BLOB_PAD;
+    float* qw = reinterpret_cast<float*>(tile + Cfg::TILE_BYTES);
+    float* qdiff = qw + TC_WG;
+    float* racc = qdiff + TC_WG * 3;
+    unsigned char* qowner = reinterpret_cast<unsigned char*>(racc + TC_WG * 3);
+    uint64_t* bar = reinterpret_cast<uint64_t*>(qowner + TC_WG);
+    const int wt = threadIdx.x;
+    const TcBlobLayout BL = tc_blob_layout(KPAD, W);
+
+    if (wt == 0) {
+        tc_mbar_init(bar, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    }
+    __syncthreads();
+    if (wt == 0) {
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" :: "r"(s_u32(bar)), "r"((uint32_t)BL.total) : "memory");
+        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
+                     :: "r"(s_u32(blob)), "l"(s.tc_blob), "r"((uint32_t)BL.total), "r"(s_u32(bar)) : "memory");
+    }
+    const long long r0 = (long long)blockIdx.x * TC_WG;
+    const int valid = (int)(n - r0 < TC_WG ? n - r0 : TC_WG);
+    const long long r = r0 + wt;
+    float f[KPAD];
+#pragma unroll
+    for (int k = 0; k < KPAD; ++k) f[k] = 0.f;
+    if (wt < valid)
+        for (int k = 0; k < s.dim0; ++k) f[__ldg(s.tc_colmap + k)] = xs[r * s.dim0 + k];
+    unsigned char* rowp = tile + tc_canon_off(wt, 0, KCH);
+#pragma unroll
+    for (int kc = 0; kc < KCH; ++kc)
+        *reinterpret_cast<uint4*>(rowp + kc * 128) = make_uint4(pack2(f[8 * kc + 0], f[8 * kc + 1]), pack2(f[8 * kc + 2], f[8 * kc + 3]),
+                                                                pack2(f[8 * kc + 4], f[8 * kc + 5]), pack2(f[8 * kc + 6], f[8 * kc + 7]));
+    qw[wt] = wt < valid ? ws[r] : 0.f;
+    qowner[wt] = (unsigned char)(wt < valid ? (owners[r] & (TC_WG - 1)) : 0);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        qdiff[3 * wt + c] = (diffs && wt < valid) ? diffs[3 * r + c] : 0.f;
+        racc[3 * wt + c] = 0.f;
+    }
+    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");      // generic smem writes -> async proxy
+    tc_mbar_wait(bar, 0);
+    __syncthreads();
+    mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0>(s_u32(tile), blob, BL, valid, 0u, qw, qowner, qdiff, racc, wt);
+    __syncthreads();
+#pragma unroll
+    for (int c = 0; c < 3; ++c) racc_out[3 * (r0 + wt) + c] = racc[3 * wt + c];
+}
+
+template <class Cfg>
+int launch_test_rgbnet_ws(const k4_scene* sc, const k4_rgbnet_test_args* a, cudaStream_t st) {
+    auto kern = k4_test_rgbnet_ws_kernel<Cfg>;
+    constexpr int smem = Cfg::BLOB_PAD + Cfg::TILE_BYTES + TC_WG * (4 + 12 + 12 + 1) + 16;
+    K4_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    const long long blocks = (a->n + TC_WG - 1) / TC_WG;
+    kern<<<(unsigned)blocks, TC_WG, smem, st>>>(sc->dev, a->d_x, a->d_diffuse, a->d_w, a->d_owner, a->n, a->d_racc);
+    K4_CUDA_TRY(cudaGetLastError());
+    return K4_OK;
+}
+
 }  // namespace
+
+int k4_testing_rgbnet_ws(const k4_scene* sc, const k4_rgbnet_test_args* a, cudaStream_t st) {
+    if (!sc->dev.tc_blob || !sc->dev.tc_colmap) return K4_ERR_UNSUPPORTED;
+    switch (sc->dev.tc_cfg) {
+#define K4_X(id, kind, C, vpe, spe, W, direct) case id: return launch_test_rgbnet_ws<TcCfg<id, kind, C, vpe, spe, W, direct>>(sc, a, st);
+        K4_WS_CFG_LIST(K4_X)
+#undef K4_X
+        default: return K4_ERR_UNSUPPORTED;
+    }
+}
 
 int k4_launch_march_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st) {
     if (!sc->dev.tc_blob) return K4_ERR_UNSUPPORTED;

@@ -81,6 +81,14 @@ class ConvTestArgs(C.Structure):
     ]
 
 
+class RgbnetTestArgs(C.Structure):
+    """k4_rgbnet_test_args: a scene's rgbnet on caller rows for the test suite (k4_testing_rgbnet)."""
+    _fields_ = [
+        ('mode', C.c_int32), ('reserved0', C.c_int32), ('n', C.c_int64),
+        ('d_x', C.c_void_p), ('d_diffuse', C.c_void_p), ('d_w', C.c_void_p), ('d_owner', C.c_void_p), ('d_racc', C.c_void_p),
+    ]
+
+
 EXPORTS = {
     'k4_abi_version': (C.c_int, []),
     'k4_status_string': (C.c_char_p, [C.c_int]),
@@ -140,6 +148,7 @@ EXPORTS = {
     'k4_make_rays': (C.c_int, [C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_int32,
                                C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'k4_testing_conv3x3': (C.c_int, [C.POINTER(ConvTestArgs), C.POINTER(C.c_int32), C.c_void_p]),
+    'k4_testing_rgbnet': (C.c_int, [C.c_void_p, C.POINTER(RgbnetTestArgs), C.POINTER(C.c_int32), C.c_void_p]),
 }
 
 if not os.path.exists(LIB_PATH):

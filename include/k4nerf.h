@@ -416,6 +416,37 @@ typedef struct k4_conv_test_args {
 } k4_conv_test_args;
 K4_API int k4_testing_conv3x3(const k4_conv_test_args* args, int32_t* kernel_used, k4_stream_t stream);
 
+/*
+ * k4_testing_rgbnet: the scene's packed rgbnet on rows the caller supplies, run by the marchers' own device code for one
+ * K4_MLP_* mode, so that a test can compare the colour MLP sample by sample with a reference.
+ *   d_x [n][dim0]: model-layout MLP inputs, the vectors the reference's rgbnet receives (rgb_feat: the k0 channels fed to
+ *   the MLP, the MPI position code, the view embedding; lib/dvgo.py:407-412, lib/dmpigo.py:374).  d_diffuse [n][3]: the
+ *   diffuse logits k0[0:3] of a DirectVoxGO model with rgbnet_direct=False, NULL for every other model.  d_w [n]: sample
+ *   weights.  d_owner [n]: the row's owner inside its group.
+ *   Rows form groups of G consecutive rows (*group_rows receives G; the last group may be partial):
+ *     K4_MLP_TCGEN05 / _WS  G = 128: one warpgroup batch of mlp_batch_wgmma; the rows are written into a ring tile through
+ *                           the column map of the scene's K4_WS_CFG_LIST entry, as fp16 with saturation
+ *     K4_MLP_F16 / _F16X3   G = 32: one warp's MmaWarpCtx, rows appended as the marcher appends them, flushed at 32 rows
+ *                           and at the end of the group
+ *     K4_MLP_FP32           G = 32: mlp_fp32, accumulated per owner in row order
+ *   Owners are in [0, G); only their low log2(G) bits are read.
+ *   d_racc [ceil(n / G)][G][3]: racc[g][j][c] = sum over the rows of group g with owner j of w * sigmoid(logit_c (+ diffuse_c)),
+ *   what the marchers accumulate into a ray.
+ *   A mode the scene's shape has no build for returns K4_ERR_UNSUPPORTED; nothing falls back to another mode.  Arguments
+ *   are checked before any CUDA call (K4_ERR_INVALID_ARG).  The call synchronises `stream`.
+ */
+typedef struct k4_rgbnet_test_args {
+    int32_t mode;                          /* K4_MLP_*                                           */
+    int32_t reserved0;
+    int64_t n;                             /* rows, 1 .. 2^24                                    */
+    const float* d_x;
+    const float* d_diffuse;
+    const float* d_w;
+    const int32_t* d_owner;
+    float* d_racc;
+} k4_rgbnet_test_args;
+K4_API int k4_testing_rgbnet(const k4_scene* scene, const k4_rgbnet_test_args* args, int32_t* group_rows, k4_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -233,6 +233,14 @@ def _early_out_counts(ids_m, ids_d, ids_a, i_end, alphainv_last, N):
     return out
 
 
+def _trace(trace, ray_id, weights, rgb_feat, diffuse):
+    """Record the surviving samples of a forward pass with an rgbnet: ray_id [S], weights [S], the rgbnet's inputs
+    rgb_feat [S, dim0] and, for rgbnet_direct=False, the diffuse logits [S, 3] added before the sigmoid (else None)."""
+    if trace is not None:
+        trace.update(ray_id=ray_id.clone(), weights=weights.clone(), rgb_feat=rgb_feat.clone(),
+                     diffuse=None if diffuse is None else diffuse.clone())
+
+
 def _add_stats(stats, ids_m, ids_d, S_c, ray_stats, ray_id_c, N):
     """S_m/S_d: visited before the early-out (what a fused marcher touches); *_all: what the
     reference's unfused pipeline touches; S_c: samples shaded (identical in both)."""
@@ -248,7 +256,7 @@ def _add_stats(stats, ids_m, ids_d, S_c, ray_stats, ray_id_c, N):
 # forward passes
 # ----------------------------------------------------------------------------------------------
 @torch.no_grad()
-def dvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, **render_kwargs):
+def dvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **render_kwargs):
     """DirectVoxGO.forward (lib/dvgo.py:327-448) at inference (global_step=None)."""
     dev = rays_o.device
     N = len(rays_o)
@@ -305,6 +313,7 @@ def dvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, **render_kwargs)
         viewdirs_emb = torch.cat([viewdirs, viewdirs_emb.sin(), viewdirs_emb.cos()], -1)
         viewdirs_emb = viewdirs_emb.flatten(0, -2)[ray_id]
         rgb_feat = torch.cat([k0_view, viewdirs_emb], -1)
+        _trace(trace, ray_id, weights, rgb_feat, None if st['rgbnet_direct'] else k0_diffuse)
         rgb_logit = mlp(st['rgbnet'], rgb_feat)
         if st['rgbnet_direct']:
             rgb_raw = torch.sigmoid(rgb_logit)
@@ -332,7 +341,7 @@ def dvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, **render_kwargs)
 
 
 @torch.no_grad()
-def dmpigo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, **render_kwargs):
+def dmpigo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **render_kwargs):
     """DirectMPIGO.forward (lib/dmpigo.py:292-427) at inference (global_step=None)."""
     dev = rays_o.device
     N = len(rays_o)
@@ -387,6 +396,7 @@ def dmpigo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, **render_kwarg
         pe_emb = (pe_spa.unsqueeze(-1) * st['posfreq']).flatten(-2)
         pe_emb = torch.cat([pe_spa, pe_emb.sin(), pe_emb.cos()], -1)
         rgb_feat = torch.cat([vox_emb, pe_emb, viewdirs_emb], -1)
+        _trace(trace, ray_id, weights, rgb_feat, None)
         rgb_logit = mlp(st['rgbnet'], rgb_feat)
         rgb_raw = torch.sigmoid(rgb_logit)
 
@@ -409,7 +419,7 @@ def dmpigo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, **render_kwarg
 
 
 @torch.no_grad()
-def dcvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, **render_kwargs):
+def dcvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **render_kwargs):
     """DirectContractedVoxGO.forward (lib/dcvgo.py:264-382, sample_ray :226-262) at inference."""
     dev = rays_o.device
     N = len(rays_o)
@@ -465,7 +475,9 @@ def dcvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, **render_kwargs
         viewdirs_emb = (viewdirs.unsqueeze(-1) * st['viewfreq']).flatten(-2)
         viewdirs_emb = torch.cat([viewdirs, viewdirs_emb.sin(), viewdirs_emb.cos()], -1)
         viewdirs_emb = viewdirs_emb.flatten(0, -2)[ray_id]
-        rgb = torch.sigmoid(mlp(st['rgbnet'], torch.cat([k0, viewdirs_emb], -1)))
+        rgb_feat = torch.cat([k0, viewdirs_emb], -1)
+        _trace(trace, ray_id, weights, rgb_feat, None)
+        rgb = torch.sigmoid(mlp(st['rgbnet'], rgb_feat))
     rgb_marched = _segment_sum(weights.unsqueeze(-1) * rgb, ray_id, torch.zeros([N, 3], device=dev))
     rgb_marched += (alphainv_last.unsqueeze(-1) * render_kwargs['bg'])
     s = 1 - 1 / (1 + tt)
@@ -479,11 +491,12 @@ def dcvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, **render_kwargs
     return ret
 
 
-def forward(st, rays_o, rays_d, viewdirs, ops, stats=None, **render_kwargs):
+def forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **render_kwargs):
+    """trace: optional dict that receives the samples shaded by the rgbnet (see _trace)."""
     if st['kind'] == 'dcvgo':
-        return dcvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=stats, **render_kwargs)
+        return dcvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=stats, trace=trace, **render_kwargs)
     fn = dvgo_forward if st['kind'] == 'dvgo' else dmpigo_forward
-    return fn(st, rays_o, rays_d, viewdirs, ops, stats=stats, **render_kwargs)
+    return fn(st, rays_o, rays_d, viewdirs, ops, stats=stats, trace=trace, **render_kwargs)
 
 
 @torch.no_grad()

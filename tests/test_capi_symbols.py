@@ -94,3 +94,37 @@ def test_testing_conv3x3_validates_arguments_without_a_gpu():
     sft = dict(mode=5, d_cond16=C.addressof(buf), h_sft=C.cast(ptrs, C.POINTER(C.c_void_p)))
     assert lib.k4_testing_conv3x3(C.byref(args(cout=16, **sft)), C.byref(used), None) == -2
     assert lib.k4_testing_conv3x3(C.byref(args(upsample2x=1, **sft)), C.byref(used), None) == -2
+
+
+def test_testing_rgbnet_validates_arguments_without_a_gpu():
+    """k4_testing_rgbnet (a scene's rgbnet on caller rows for the GPU tests): bad arguments are reported as
+    K4_ERR_INVALID_ARG before any CUDA call, and *group_rows stays 0.  The scene here is a zero-filled host block: a scene
+    without an MLP, whose every mode is K4_ERR_UNSUPPORTED once the arguments are valid."""
+    from k4nerf import _lib
+    C = ctypes
+    lib = _lib.lib
+    A = _lib.RgbnetTestArgs
+    assert C.sizeof(A) == 56 and A.n.offset == 8 and A.d_x.offset == 16 and A.d_racc.offset == 48     # the header's layout
+    buf = C.create_string_buffer(64)
+    scene = C.create_string_buffer(1 << 16)           # zeros: kind DVGO, rgbnet_direct 0 -> d_diffuse required
+
+    def args(**kw):
+        a = A()
+        a.mode, a.n = _lib.K4_MLP_F16, 33
+        a.d_x = a.d_diffuse = a.d_w = a.d_owner = a.d_racc = C.addressof(buf)
+        for k, v in kw.items():
+            setattr(a, k, v)
+        return a
+
+    g = C.c_int32(7)
+    bad = [dict(mode=-1), dict(mode=5), dict(n=0), dict(n=-3), dict(n=(1 << 24) + 1), dict(d_x=None), dict(d_w=None),
+           dict(d_owner=None), dict(d_racc=None), dict(d_diffuse=None)]
+    for kw in bad:
+        g.value = 7
+        assert lib.k4_testing_rgbnet(C.addressof(scene), C.byref(args(**kw)), C.byref(g), None) == -1, kw
+        assert g.value == 0, kw
+    assert lib.k4_testing_rgbnet(None, C.byref(args()), C.byref(g), None) == -1
+    assert lib.k4_testing_rgbnet(C.addressof(scene), None, C.byref(g), None) == -1
+    for mode in range(5):
+        assert lib.k4_testing_rgbnet(C.addressof(scene), C.byref(args(mode=mode)), C.byref(g), None) == -2, mode
+        assert g.value == 0
