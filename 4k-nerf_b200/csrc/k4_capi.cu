@@ -84,13 +84,14 @@ __global__ void pack_w_f16_kernel(const float* __restrict__ W, __half* __restric
 // wgmma operand tiles (canonical K-major, no swizzle; see tc_canon_off)
 // The destination tile is pre-zeroed; model weight (n, k) lands at column colmap[k] (identity when colmap == nullptr):
 // the config's row layout may hold more inputs than the model has (k4_ws_cfgs.h), those columns stay zero.
+// output n of the layer goes to operand row n * rstride (the rows between stay as the caller zeroed them)
 __global__ void pack_tc_weight_kernel(const float* __restrict__ W, unsigned char* __restrict__ dst,
-                                      int n_out, int n_in, int kpad, const int* __restrict__ colmap) {
+                                      int n_out, int n_in, int kpad, const int* __restrict__ colmap, int rstride = 1) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_out * n_in) return;
     const int n = i / n_in, k = i - n * n_in;
     const int kd = colmap ? colmap[k] : k;
-    *reinterpret_cast<__half*>(dst + tc_canon_off(n, kd >> 3, kpad >> 3) + (kd & 7) * 2) = __float2half_rn(W[i]);
+    *reinterpret_cast<__half*>(dst + tc_canon_off(n * rstride, kd >> 3, kpad >> 3) + (kd & 7) * 2) = __float2half_rn(W[i]);
 }
 
 // ---- empty-space skipping: coarse occupancy of the mask and its Chebyshev distance field ----
@@ -123,13 +124,14 @@ __global__ void skip_cap_kernel(uint8_t* __restrict__ dist, int n) {
     if (c < n && dist[c] == 255) dist[c] = K4_SKIP_MAXD + 1;
 }
 // bias tile [npad][16]: col 0 = fp16(b), col 1 = fp16(b - col0); multiplied by the ONES tile (cols 0,1 = 1)
-__global__ void pack_tc_bias_kernel(const float* __restrict__ b, unsigned char* __restrict__ dst, int n_out, int npad) {
+// output j of the layer goes to row j * rstride of the npad-row tile; every other row is zero
+__global__ void pack_tc_bias_kernel(const float* __restrict__ b, unsigned char* __restrict__ dst, int n_out, int npad, int rstride = 1) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= npad * 16) return;
     const int n = i / 16, k = i - n * 16;
     float v = 0.f;
-    if (n < n_out && k < 2) {
-        const float bb = b[n];
+    if (n % rstride == 0 && n / rstride < n_out && k < 2) {
+        const float bb = b[n / rstride];
         const __half hi = __float2half_rn(bb);
         v = (k == 0) ? __half2float(hi) : (bb - __half2float(hi));
     }
@@ -409,10 +411,11 @@ extern "C" int k4_scene_create(const k4_scene_desc* d, k4_stream_t stream, k4_sc
                 const int wm = v.width;
                 pack_tc_weight_kernel<<<(wm * dim0 + 255) / 256, 256, 0, s>>>(d->d_rgbnet_weight[0], blob + BL.off_w1, wm, dim0, kpad, d_colmap);
                 pack_tc_weight_kernel<<<(wm * wm + 255) / 256, 256, 0, s>>>(d->d_rgbnet_weight[1], blob + BL.off_w2, wm, wm, w, nullptr);
-                pack_tc_weight_kernel<<<(3 * wm + 255) / 256, 256, 0, s>>>(d->d_rgbnet_weight[2], blob + BL.off_w3, 3, wm, w, nullptr);
+                // W3 / B3: output channel c at operand row (accumulator column) 2c, for mlp_batch_wgmma's epilogue
+                pack_tc_weight_kernel<<<(3 * wm + 255) / 256, 256, 0, s>>>(d->d_rgbnet_weight[2], blob + BL.off_w3, 3, wm, w, nullptr, 2);
                 pack_tc_bias_kernel<<<(w * 16 + 255) / 256, 256, 0, s>>>(d->d_rgbnet_bias[0], blob + BL.off_b1, wm, w);
                 pack_tc_bias_kernel<<<(w * 16 + 255) / 256, 256, 0, s>>>(d->d_rgbnet_bias[1], blob + BL.off_b2, wm, w);
-                pack_tc_bias_kernel<<<1, 256, 0, s>>>(d->d_rgbnet_bias[2], blob + BL.off_b3, 3, 16);
+                pack_tc_bias_kernel<<<1, 256, 0, s>>>(d->d_rgbnet_bias[2], blob + BL.off_b3, 3, 16, 2);
                 pack_tc_ones_kernel<<<8, 256, 0, s>>>(blob + BL.off_ones);
                 K4_CTRY(cudaGetLastError());
                 v.tc_blob = blob; v.tc_kpad = kpad; v.tc_width = w; v.tc_cfg = c.id; v.tc_colmap = d_colmap;
@@ -431,10 +434,12 @@ extern "C" int k4_scene_create(const k4_scene_desc* d, k4_stream_t stream, k4_sc
 // ------------------------------------------------------------------------------------------------
 extern "C" size_t k4_render_workspace_bytes(const k4_scene*, int64_t) { return 256; }
 
+// phases != NULL: the profiled ws marcher of k4_testing_march_phases (room for max_ctas CTAs, count to *n_ctas)
 static int render_impl(const k4_scene* sc, const k4_render_args* a,
                        const float* d_rays_o, const float* d_rays_d, const float* d_viewdirs,
                        int64_t n_rays, const k4_render_out* out, const k4_frame_dst* fd,
-                       void* d_workspace, size_t workspace_bytes, k4_stream_t stream) {
+                       void* d_workspace, size_t workspace_bytes, k4_stream_t stream,
+                       unsigned long long* phases = nullptr, int max_ctas = 0, int* n_ctas = nullptr) {
     static const k4_render_out no_out = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     if (!sc || !a || (!out && !fd)) return K4_ERR_INVALID_ARG;
     if (!out) out = &no_out;
@@ -501,7 +506,7 @@ static int render_impl(const k4_scene* sc, const k4_render_args* a,
     K4_CUDA_TRY(cudaMemsetAsync(d_workspace, 0, 16, s));
     if ((a->mlp_mode == K4_MLP_TCGEN05 || a->mlp_mode == K4_MLP_TCGEN05_WS) && v.depth > 0) {
         if (a->mlp_mode == K4_MLP_TCGEN05) return k4_tc_supported(v) ? k4_launch_march_tc(sc, rp, s) : K4_ERR_UNSUPPORTED;
-        return k4_ws_supported(v) ? k4_launch_march_ws(sc, rp, s) : K4_ERR_UNSUPPORTED;
+        return k4_ws_supported(v) ? k4_launch_march_ws(sc, rp, s, phases, max_ctas, n_ctas) : K4_ERR_UNSUPPORTED;
     }
     return k4_launch_march(sc, rp, a->mlp_mode, s);
 }
@@ -512,6 +517,21 @@ extern "C" int k4_render_rays(const k4_scene* sc, const k4_render_args* a,
                               void* d_workspace, size_t workspace_bytes, k4_stream_t stream) {
     if (!out) return K4_ERR_INVALID_ARG;
     return render_impl(sc, a, d_rays_o, d_rays_d, d_viewdirs, n_rays, out, nullptr, d_workspace, workspace_bytes, stream);
+}
+
+extern "C" int k4_testing_march_phases(const k4_scene* sc, const k4_render_args* a,
+                                       const float* d_rays_o, const float* d_rays_d, const float* d_viewdirs,
+                                       int64_t n_rays, const k4_render_out* out, void* d_workspace, size_t workspace_bytes,
+                                       uint64_t* d_phases, int32_t max_ctas, int32_t* n_ctas, k4_stream_t stream) {
+    if (n_ctas) *n_ctas = 0;
+    if (!sc || !a || !out || !d_phases || max_ctas < 1 || n_rays < 1) return K4_ERR_INVALID_ARG;
+    if (a->mlp_mode != K4_MLP_TCGEN05_WS) return K4_ERR_INVALID_ARG;
+    if (sc->dev.depth == 0) return K4_ERR_UNSUPPORTED;
+    int n = 0;
+    const int st = render_impl(sc, a, d_rays_o, d_rays_d, d_viewdirs, n_rays, out, nullptr, d_workspace, workspace_bytes, stream,
+                               reinterpret_cast<unsigned long long*>(d_phases), max_ctas, &n);
+    if (st == K4_OK && n_ctas) *n_ctas = n;
+    return st;
 }
 
 extern "C" int k4_render_rays_frames(const k4_scene* sc, const k4_render_args* a,

@@ -29,13 +29,49 @@ __device__ __forceinline__ void mlp_repack(const float (&acc)[32], uint32_t (*h)
     }
 }
 
+// Phase accounting of the profiled ws marcher (k4_testing_march_phases): mark(p) charges the SM cycles since the previous
+// mark to counter p (K4_PH_*) of the warpgroup.  Thread 0 of the group keeps the clock and the counters in shared memory.
+// NoPhases, the marker of every production kernel, compiles to nothing.
+struct NoPhases {
+    __device__ __forceinline__ void operator()(int) const {}
+};
+struct PhaseClock {
+    static constexpr int START = K4_PHASE_SLOTS, LAST = K4_PHASE_SLOTS + 1, WORDS = K4_PHASE_SLOTS + 2;
+    unsigned long long* ctr;     // [WORDS]: the counters, the group's start, the previous mark
+    bool on;                     // thread 0 of the warpgroup
+    __device__ __forceinline__ static unsigned long long now() {
+        unsigned long long t;
+        asm volatile("mov.u64 %0, %%clock64;\n" : "=l"(t) :: "memory");
+        return t;
+    }
+    __device__ __forceinline__ void begin() const {
+        if (!on) return;
+        for (int i = 0; i < K4_PHASE_SLOTS; ++i) ctr[i] = 0ull;
+        ctr[START] = ctr[LAST] = now();
+    }
+    __device__ __forceinline__ void operator()(int p) const {
+        if (!on) return;
+        const unsigned long long t = now();
+        ctr[p] += t - ctr[LAST];
+        ctr[LAST] = t;
+    }
+    // the elapsed cycles and the batch count into slots K4_PH_ELAPSED / 7, all slots to out[0 .. K4_PHASE_SLOTS)
+    __device__ __forceinline__ void end(unsigned long long batches, unsigned long long* out) const {
+        if (!on) return;
+        ctr[K4_PH_ELAPSED] = ctr[LAST] - ctr[START];
+        ctr[K4_PHASE_SLOTS - 1] = batches;
+        for (int i = 0; i < K4_PHASE_SLOTS; ++i) out[i] = ctr[i];
+    }
+};
+
 // Rows [0, valid) of the ring tile at shared address a_tile (canonical K-major, KPAD/8 chunks per row).  Row r is
 // queue slot slot0 + r: its colour, weighted by qw[slot], is added to racc[3 * qowner[slot] + c].  Called by all 128
-// threads of one warpgroup (wt = thread index in the group); `valid` must be the same for all of them.
-template <int W, int KPAD, bool DIRECT>
+// threads of one warpgroup (wt = thread index in the group); `valid` must be the same for all of them.  `mark` receives
+// the phase boundaries (PhaseClock).
+template <int W, int KPAD, bool DIRECT, class Mark = NoPhases>
 __device__ __forceinline__ void mlp_batch_wgmma(uint32_t a_tile, const unsigned char* blob, const TcBlobLayout& BL, int valid,
                                                 unsigned slot0, const float* qw, const unsigned char* qowner, const float* qdiff,
-                                                float* racc, int wt) {
+                                                float* racc, int wt, const Mark& mark = Mark()) {
     constexpr int KCH = KPAD / 8, KCHW = W / 8, NC = W / 64;      // NC: 64-column blocks of a hidden layer
     static_assert(W % 64 == 0, "hidden width");
     const int warp = wt >> 5, lane = wt & 31, g = lane >> 2, t = lane & 3;
@@ -60,8 +96,10 @@ __device__ __forceinline__ void mlp_batch_wgmma(uint32_t a_tile, const unsigned 
             wg_commit();
             wg_wait<0>();
             wg_fence_acc(acc);
+            mark(K4_PH_L_L1);
 #pragma unroll
             for (int nc = 0; nc < NC; ++nc) mlp_repack(*reinterpret_cast<const float (*)[32]>(acc + 32 * nc), h1 + 4 * nc);
+            mark(K4_PH_L_REPACK);
         }
         {
             float acc[W / 2];
@@ -72,8 +110,10 @@ __device__ __forceinline__ void mlp_batch_wgmma(uint32_t a_tile, const unsigned 
             wg_commit();
             wg_wait<0>();
             wg_fence_acc(acc);
+            mark(K4_PH_L_L2);
 #pragma unroll
             for (int nc = 0; nc < NC; ++nc) mlp_repack(*reinterpret_cast<const float (*)[32]>(acc + 32 * nc), h2 + 4 * nc);
+            mark(K4_PH_L_REPACK);
         }
         float o[8];
         wg_fence();
@@ -83,25 +123,21 @@ __device__ __forceinline__ void mlp_batch_wgmma(uint32_t a_tile, const unsigned 
         wg_commit();
         wg_wait<0>();
         wg_fence_acc(o);
-        // logits 0, 1 of rows g / g+8 sit in lane t = 0, logit 2 in lane t = 1
-        const float l2a = __shfl_down_sync(FULL, o[0], 1), l2b = __shfl_down_sync(FULL, o[2], 1);
-        if (t == 0) {
+        mark(K4_PH_L_L3);
+        // W3 / B3 hold output channel c in column 2c (k4_scene_create), so channel c of rows g / g+8 is o[0] / o[2] of lane
+        // t = c: three lanes of each quad share the epilogue, two sigmoids and two atomics each
+        if (t < 3) {
 #pragma unroll
             for (int rr = 0; rr < 2; ++rr) {
                 const int row = mh * 64 + warp * 16 + g + 8 * rr;
                 if (row < valid) {
                     const unsigned slot = slot0 + (unsigned)row;
-                    const float wq = qw[slot];
-                    const int owner = qowner[slot];
-                    const float lg[3] = {o[2 * rr], o[2 * rr + 1], rr ? l2b : l2a};
-#pragma unroll
-                    for (int ch = 0; ch < 3; ++ch) {
-                        float logit = lg[ch];
-                        if (!DIRECT) logit = __fadd_rn(logit, qdiff[slot * 3 + ch]);      // rgb_logit + k0_diffuse
-                        atomicAdd(racc + owner * 3 + ch, wq * sigmoid_ref(logit));
-                    }
+                    float logit = o[2 * rr];
+                    if (!DIRECT) logit = __fadd_rn(logit, qdiff[slot * 3 + t]);      // rgb_logit + k0_diffuse
+                    atomicAdd(racc + qowner[slot] * 3 + t, qw[slot] * sigmoid_ref(logit));
                 }
             }
         }
+        mark(K4_PH_L_EPILOGUE);
     }
 }

@@ -58,6 +58,7 @@ struct TcCfg {
     static constexpr int WG_BYTES = (WG_MISC + 128 + 1023) & ~1023;
     static constexpr int CTA_MISC = BLOB_PAD + 2 * WG_BYTES; // weight mbarrier
     static constexpr int SMEM = CTA_MISC + 64;
+    static constexpr int PROF_SMEM = SMEM + 4 * PhaseClock::WORDS * 8;   // + the phase counters of the profiled kernel
 };
 
 __device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -112,9 +113,11 @@ struct WgCtl {
     uint64_t done_bar;             // MLP -> marcher: a batch has been consumed      (count 128)
 };
 
-template <class Cfg>
+// PROF: the profiled instantiation (k4_testing_march_phases).  It adds the phase marks of PhaseClock and nothing else, and
+// writes each warpgroup's counters to phases[(blockIdx.x * 4 + wg) * K4_PHASE_SLOTS ..].
+template <class Cfg, bool PROF>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4RenderParams rp) {
+k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4RenderParams rp, unsigned long long* phases) {
     extern __shared__ __align__(1024) unsigned char smem[];
     constexpr int W = Cfg::W, KPAD = Cfg::KPAD, KCH = Cfg::KCH;
     const int tid = threadIdx.x, wg = tid >> 7, wt = tid & 127, lane = tid & 31, warp_in_wg = wt >> 5;
@@ -147,6 +150,9 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
                      :: "r"(s_u32(blob)), "l"(s.tc_blob), "r"((uint32_t)BL.total), "r"(s_u32(wbar)) : "memory");
     }
     tc_mbar_wait(wbar, 0);
+    const PhaseClock clk{reinterpret_cast<unsigned long long*>(smem + Cfg::SMEM) + wg * PhaseClock::WORDS, PROF && wt == 0};
+    auto mark = [&](int p) { if (PROF) clk(p); };
+    if (PROF) clk.begin();
 
     if (wg >= 2) {
         // =====================================================================================
@@ -164,16 +170,22 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
         unsigned long long n_batches = 0;
         for (;;) {
             tc_mbar_wait(&c->full_bar, full_ph); full_ph ^= 1;
+            mark(K4_PH_L_WAIT_FULL);
             if (*reinterpret_cast<volatile unsigned int*>(&c->exit_flag)) break;
             const unsigned tile = nb % TC_TILES;
             if (wt == 0) ++n_batches;
             const int valid = *reinterpret_cast<volatile int*>(&c->valid[tile]);
-            mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0>(ring_s + tile * Cfg::TILE_BYTES, blob, BL, valid, tile * 128u, qw, qowner, qdiff,
-                                                       racc, wt);
+            if (PROF)
+                mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0>(ring_s + tile * Cfg::TILE_BYTES, blob, BL, valid, tile * 128u, qw, qowner,
+                                                           qdiff, racc, wt, clk);
+            else
+                mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0>(ring_s + tile * Cfg::TILE_BYTES, blob, BL, valid, tile * 128u, qw, qowner,
+                                                           qdiff, racc, wt);
             mbar_arrive(&c->done_bar);              // 128 arrivals = batch consumed
             ++nb;
         }
         if (rp.counters && wt == 0) atomicAdd(rp.counters + 3, n_batches);
+        if (PROF) clk.end(n_batches, phases + ((size_t)blockIdx.x * 4 + wg) * K4_PHASE_SLOTS);
     } else {
         // =====================================================================================
         // marcher warpgroups
@@ -203,7 +215,9 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
         auto submit = [&](int valid) {
             asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");      // generic smem writes -> async proxy
             named_bar(wg + 1);
+            mark(K4_PH_M_RENDEZVOUS);
             while (n_done < n_sub) { tc_mbar_wait(&ctl->done_bar, done_ph); done_ph ^= 1; ++n_done; }
+            mark(K4_PH_M_WAIT_DONE);
             if (wt == 0) {
                 *reinterpret_cast<volatile int*>(&ctl->valid[n_sub % TC_TILES]) = valid;
                 __threadfence_block();
@@ -289,6 +303,7 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
                 for (int j = 0; j < Cfg::NVW; ++j) vw[j] = pack2(ve[2 * j], ve[2 * j + 1]);
             }
 
+            mark(K4_PH_M_SETUP);
             float T = 1.f, acc_depth = 0.f;
             int cnt_m = 0, cnt_d = 0, cnt_c = 0;
             bool done = !have_ray;
@@ -438,7 +453,9 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
                     }
                 }
                 // ---------------- warpgroup rendezvous ----------------
+                mark(K4_PH_M_MARCH);
                 const bool live = wg_bar_or(wg, !done && (i < r.n_steps));
+                mark(K4_PH_M_RENDEZVOUS);
                 const unsigned tail = *tailp;                          // stable until the next barrier
                 if (tail - head >= 128u) {
                     submit(128);
@@ -447,15 +464,18 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
                         submit((int)(tail - head));
                         named_bar(wg + 1);                             // everyone has read `tail`
                         if (wt == 0) *tailp = head;
+                        mark(K4_PH_M_RENDEZVOUS);
                     }
                     break;
                 } else {
                     named_bar(wg + 1);
+                    mark(K4_PH_M_RENDEZVOUS);
                 }
             }
             // all of this tile's batches must be consumed before the accumulators are read
             while (n_done < n_sub) { tc_mbar_wait(&ctl->done_bar, done_ph); done_ph ^= 1; ++n_done; }
             named_bar(wg + 1);
+            mark(K4_PH_M_DRAIN);
             if (have_ray) {
                 const float bgt = __fmul_rn(T, rp.bg);
                 k4_store_ray(rp, ray_i, __fadd_rn(racc[wt * 3 + 0], bgt), __fadd_rn(racc[wt * 3 + 1], bgt),
@@ -465,6 +485,7 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
             }
             racc[wt * 3 + 0] = 0.f; racc[wt * 3 + 1] = 0.f; racc[wt * 3 + 2] = 0.f;
             tot_m += cnt_m; tot_d += cnt_d; tot_c += cnt_c;
+            mark(K4_PH_M_STORE);
         }
         if (wt == 0) {   // all batches are consumed: release this slot's MLP group
             *reinterpret_cast<volatile unsigned int*>(&ctl->exit_flag) = 1u;
@@ -484,13 +505,16 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
                 atomicAdd(rp.counters + 2, tot_c);
             }
         }
+        mark(K4_PH_M_SETUP);
+        if (PROF) clk.end(n_sub, phases + ((size_t)blockIdx.x * 4 + wg) * K4_PHASE_SLOTS);
     }
 }
 
+// phases: NULL for the production kernel, else the profiled one writes there (room for max_ctas CTAs); *n_ctas: CTAs launched
 template <class Cfg>
-int launch_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st) {
-    auto kern = k4_march_ws_kernel<Cfg>;
-    K4_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
+int launch_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st, unsigned long long* phases, int max_ctas, int* n_ctas) {
+    auto kern = phases ? k4_march_ws_kernel<Cfg, true> : k4_march_ws_kernel<Cfg, false>;
+    const int smem = phases ? Cfg::PROF_SMEM : Cfg::SMEM;
     int dev = 0, sms = 0;
     K4_CUDA_TRY(cudaGetDevice(&dev));
     K4_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -499,7 +523,10 @@ int launch_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st) {
     long long blocks = (rp.n_tiles + 1) / 2;
     if (blocks > sms) blocks = sms;                     // persistent: one CTA per SM
     if (blocks < 1) blocks = 1;
-    kern<<<(unsigned)blocks, TC_THREADS, Cfg::SMEM, st>>>(sc->dev, rp);
+    if (phases && blocks > max_ctas) return K4_ERR_INVALID_ARG;
+    if (n_ctas) *n_ctas = (int)blocks;
+    K4_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    kern<<<(unsigned)blocks, TC_THREADS, smem, st>>>(sc->dev, rp, phases);
     K4_CUDA_TRY(cudaGetLastError());
     return K4_OK;
 }
@@ -585,10 +612,11 @@ int k4_testing_rgbnet_ws(const k4_scene* sc, const k4_rgbnet_test_args* a, cudaS
     }
 }
 
-int k4_launch_march_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st) {
+int k4_launch_march_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st, unsigned long long* phases, int max_ctas, int* n_ctas) {
     if (!sc->dev.tc_blob) return K4_ERR_UNSUPPORTED;
     switch (sc->dev.tc_cfg) {
-#define K4_X(id, kind, C, vpe, spe, W, direct) case id: return launch_ws<TcCfg<id, kind, C, vpe, spe, W, direct>>(sc, rp, st);
+#define K4_X(id, kind, C, vpe, spe, W, direct) \
+        case id: return launch_ws<TcCfg<id, kind, C, vpe, spe, W, direct>>(sc, rp, st, phases, max_ctas, n_ctas);
         K4_WS_CFG_LIST(K4_X)
 #undef K4_X
         default: return K4_ERR_UNSUPPORTED;

@@ -81,6 +81,12 @@ class ConvTestArgs(C.Structure):
     ]
 
 
+# k4_testing_march_phases: counters per warpgroup and their slots (marchers: K4_PH_M_*, MLP groups: K4_PH_L_*)
+K4_PHASE_SLOTS = 8
+MARCHER_PHASES = {1: 'setup', 2: 'march', 3: 'rendezvous', 4: 'wait_done', 5: 'drain', 6: 'store'}
+MLP_PHASES = {1: 'wait_full', 2: 'l1', 3: 'l2', 4: 'l3', 5: 'repack', 6: 'epilogue'}
+
+
 class RgbnetTestArgs(C.Structure):
     """k4_rgbnet_test_args: a scene's rgbnet on caller rows for the test suite (k4_testing_rgbnet)."""
     _fields_ = [
@@ -149,6 +155,9 @@ EXPORTS = {
                                C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'k4_testing_conv3x3': (C.c_int, [C.POINTER(ConvTestArgs), C.POINTER(C.c_int32), C.c_void_p]),
     'k4_testing_rgbnet': (C.c_int, [C.c_void_p, C.POINTER(RgbnetTestArgs), C.POINTER(C.c_int32), C.c_void_p]),
+    'k4_testing_march_phases': (C.c_int, [C.c_void_p, C.POINTER(RenderArgs), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                          C.POINTER(RenderOut), C.c_void_p, C.c_size_t, C.c_void_p, C.c_int32,
+                                          C.POINTER(C.c_int32), C.c_void_p]),
 }
 
 if not os.path.exists(LIB_PATH):

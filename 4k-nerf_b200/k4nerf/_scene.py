@@ -180,13 +180,16 @@ class FusedRenderMixin:
 
     @torch.no_grad()
     def render_rays(self, rays_o, rays_d, viewdirs, render_kwargs, image_hw=None, mlp_mode=None,
-                    debug=False, out=None):
+                    debug=False, out=None, phases=None):
         """Run the fused kernel.  Returns dict(rgb_marched, alphainv_last[, depth][, ray_stats, t_minmax, counters]).
         ``out``: optional dict of caller-owned contiguous fp32 CUDA tensors ``rgb_marched [N,3]``, ``alphainv_last [N]``
         (and ``depth [N]``) the kernel writes into -- e.g. views of a packed communication buffer (k4nerf.dist) -- or a
         :class:`k4nerf.dist.FrameTarget`: the rays are one rank's rows of a block-cyclic multi-GPU frame and every ray is
         stored straight into every rank's image-order frame (k4_render_rays_frames); the returned dict then holds only
-        the debug outputs."""
+        the debug outputs.
+        ``phases``: a contiguous int64 CUDA tensor [max_ctas, 4, K4_PHASE_SLOTS]; the 'ws' kernel then runs in its profiled
+        instantiation (k4_testing_march_phases), which fills the tensor's first ``ret['n_ctas']`` rows with the phase
+        cycles of every warpgroup."""
         assert rays_o.dim() == 2 and rays_o.shape[-1] == 3, 'Only suuport point queries in [N, 3] format'
         require_cuda(rays_o, rays_d, viewdirs)
         h = self._get_scene()
@@ -248,7 +251,17 @@ class FusedRenderMixin:
             object.__setattr__(self, '_k4_ws', ws)
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev).cuda_stream
-            if frames is not None:
+            if phases is not None:
+                if frames is not None or not (phases.is_cuda and phases.dtype == torch.int64 and phases.is_contiguous()
+                                              and phases.dim() == 3 and tuple(phases.shape[1:]) == (4, _lib.K4_PHASE_SLOTS)):
+                    raise ValueError('render_rays(phases=...): an int64 CUDA tensor [max_ctas, 4, K4_PHASE_SLOTS], no FrameTarget')
+                n_ctas = C.c_int32(0)
+                _lib.check(_lib.lib.k4_testing_march_phases(h.ptr, C.byref(a), rays_o.data_ptr(), rays_d.data_ptr(),
+                                                            viewdirs.data_ptr(), N, C.byref(o), ws.data_ptr(), ws.numel(),
+                                                            phases.data_ptr(), phases.shape[0], C.byref(n_ctas),
+                                                            C.c_void_p(stream)), 'k4_testing_march_phases')
+                ret['n_ctas'] = n_ctas.value
+            elif frames is not None:
                 _lib.check(_lib.lib.k4_render_rays_frames(h.ptr, C.byref(a), rays_o.data_ptr(), rays_d.data_ptr(),
                                                           viewdirs.data_ptr(), N, C.byref(frames), C.byref(o), ws.data_ptr(),
                                                           ws.numel(), C.c_void_p(stream)), 'k4_render_rays_frames')

@@ -447,6 +447,41 @@ typedef struct k4_rgbnet_test_args {
 } k4_rgbnet_test_args;
 K4_API int k4_testing_rgbnet(const k4_scene* scene, const k4_rgbnet_test_args* args, int32_t* group_rows, k4_stream_t stream);
 
+/*
+ * k4_testing_march_phases: k4_render_rays in mode K4_MLP_TCGEN05_WS, run by the profiled instantiation of the
+ * warp-specialised marcher.  It computes what the production kernel computes and, besides, where each warpgroup's SM
+ * cycles go: thread 0 of every warpgroup reads the SM clock at each phase boundary and charges the cycles since the
+ * previous boundary to the phase that ended, so a warpgroup's phases add up to its elapsed cycles.
+ *   d_phases [n_ctas][4][K4_PHASE_SLOTS] uint64: CTA c, warpgroup g (0, 1 marchers; 2, 3 the MLP groups of marchers
+ *   0, 1), slots K4_PH_* below.  max_ctas: CTAs d_phases has room for; the launch has min(SM count, ceil(tiles / 2))
+ *   CTAs, and a launch that needs more returns K4_ERR_INVALID_ARG before it starts.  *n_ctas receives the CTA count.
+ *   Every other argument has k4_render_rays' meaning; args->mlp_mode must be K4_MLP_TCGEN05_WS.  Arguments are checked
+ *   before any CUDA call (K4_ERR_INVALID_ARG), except the CTA count, which needs the device's SM count.  Does not
+ *   synchronise `stream`.
+ */
+enum { K4_PHASE_SLOTS = 8 };
+enum { K4_PH_ELAPSED = 0,                  /* every warpgroup: cycles from the staged weights to its exit              */
+       /* marcher warpgroups */
+       K4_PH_M_SETUP = 1,                  /*   tile fetch, ray setup, exit                                            */
+       K4_PH_M_MARCH = 2,                  /*   stepping, gathers, appending rows to the ring                          */
+       K4_PH_M_RENDEZVOUS = 3,             /*   warpgroup barriers between marching rounds and before a submit         */
+       K4_PH_M_WAIT_DONE = 4,              /*   submit: waiting until the MLP group has consumed the previous batch    */
+       K4_PH_M_DRAIN = 5,                  /*   tile end: waiting until every batch of the tile is consumed            */
+       K4_PH_M_STORE = 6,                  /*   tile end: storing the rays                                             */
+       K4_PH_M_BATCHES = 7,                /*   count: batches submitted                                               */
+       /* MLP warpgroups */
+       K4_PH_L_WAIT_FULL = 1,              /*   waiting for a batch (FULL), or for the exit                            */
+       K4_PH_L_L1 = 2,                     /*   waiting for layer 1's MMAs (issue to retire)                           */
+       K4_PH_L_L2 = 3,
+       K4_PH_L_L3 = 4,
+       K4_PH_L_REPACK = 5,                 /*   accumulators -> ReLU'd fp16 operands of the next layer                 */
+       K4_PH_L_EPILOGUE = 6,               /*   sigmoid, weight and shared-memory atomics into the rays                */
+       K4_PH_L_BATCHES = 7 };              /*   count: batches consumed                                                */
+K4_API int k4_testing_march_phases(const k4_scene* scene, const k4_render_args* args,
+                                   const float* d_rays_o, const float* d_rays_d, const float* d_viewdirs,
+                                   int64_t n_rays, const k4_render_out* out, void* d_workspace, size_t workspace_bytes,
+                                   uint64_t* d_phases, int32_t max_ctas, int32_t* n_ctas, k4_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
