@@ -823,7 +823,7 @@ __global__ void __launch_bounds__(128) condnet_kernel(const __grid_constant__ Co
 #pragma unroll
         for (int k = 0; k < 64; ++k) v = fmaf(c6[o * 64 + k], a[k], v);
         p.cond_out[pix * 32 + o] = v;
-        if (p.cond16) p.cond16[pix * 32 + o] = __float2half_rn(v);         // operand of the fused SFT epilogues
+        if (p.cond16) p.cond16[pix * 32 + o] = __low2half(sr_h2sat(v, 0.f));   // operand of the fused SFT epilogues, saturated
     }
 }
 
@@ -865,13 +865,14 @@ __global__ void pack_condnet_mma_kernel(const float* __restrict__ w, unsigned ch
 
 struct CondMmaParams { const float* cond_in; const unsigned char* wblk; float* cond_out; __half* cond16; int H, W, y_lo, y_hi; };
 
-// accumulator fragments of 2 adjacent n8 blocks -> hi / lo A fragments of one k16 step
+// accumulator fragments of 2 adjacent n8 blocks -> hi / lo A fragments of one k16 step.  Both halves saturate: beyond
+// the fp16 range hi = +-65504 and lo = x - hi, itself clamped, so an activation of 65520 or more stays finite (a
+// rounding to inf would make lo = -inf and the next MMA NaN).
 __device__ __forceinline__ void cnm_split_frag(const float (&c0)[4], const float (&c1)[4], uint32_t (&ah)[4], uint32_t (&al)[4]) {
     auto pk = [](float x, float y, uint32_t& hi, uint32_t& lo) {
-        const __half2 h = __floats2half2_rn(x, y);
-        const float2 hf = __half22float2(h);
-        const __half2 l = __floats2half2_rn(x - hf.x, y - hf.y);
-        hi = *reinterpret_cast<const uint32_t*>(&h); lo = *reinterpret_cast<const uint32_t*>(&l);
+        hi = sr_pack_sat(x, y);
+        const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+        lo = sr_pack_sat(x - hf.x, y - hf.y);
     };
     pk(c0[0], c0[1], ah[0], al[0]); pk(c0[2], c0[3], ah[1], al[1]);
     pk(c1[0], c1[1], ah[2], al[2]); pk(c1[2], c1[3], ah[3], al[3]);
@@ -965,11 +966,11 @@ __global__ void __launch_bounds__(128) condnet_mma_kernel(const __grid_constant_
             const int ch = 8 * j + 2 * tq;
             if (inA) {
                 *reinterpret_cast<float2*>(p.cond_out + pixA * 32 + ch) = make_float2(o[j][0], o[j][1]);
-                if (p.cond16) *reinterpret_cast<__half2*>(p.cond16 + pixA * 32 + ch) = __floats2half2_rn(o[j][0], o[j][1]);
+                if (p.cond16) *reinterpret_cast<__half2*>(p.cond16 + pixA * 32 + ch) = sr_h2sat(o[j][0], o[j][1]);
             }
             if (inB) {
                 *reinterpret_cast<float2*>(p.cond_out + pixB * 32 + ch) = make_float2(o[j][2], o[j][3]);
-                if (p.cond16) *reinterpret_cast<__half2*>(p.cond16 + pixB * 32 + ch) = __floats2half2_rn(o[j][2], o[j][3]);
+                if (p.cond16) *reinterpret_cast<__half2*>(p.cond16 + pixB * 32 + ch) = sr_h2sat(o[j][2], o[j][3]);
             }
         }
     }
@@ -1157,6 +1158,23 @@ int make_sft(k4_srnet* n, SrSft& f, const float* const* pw, int cout, cudaStream
     if (st) return st;
     K4_CUDA_TRY(cudaMemsetAsync(f.frag, 0, FL.total, s));
     pack_sft_frag_kernel<<<8, 256, 0, s>>>(f.w, f.frag, cout);
+    K4_CUDA_TRY(cudaGetLastError());
+    return K4_OK;
+}
+
+// CondNet weights: the 8 tensors of CondNet.0 (64x1x3x3), .2 (64x64), .4 (64x64), .6 (32x64) and their biases -> the fp32
+// block of condnet_kernel and the cnm_layout block of condnet_mma_kernel
+int make_condnet(k4_srnet* n, const float* const* pw, cudaStream_t s) {
+    const size_t nw = 64 * 9 + 64 + 2 * (64 * 64 + 64) + 32 * 64 + 32;
+    int st = sr_alloc(n, (void**)&n->condnet_w, nw * 4);
+    if (st) return st;
+    float* dd = n->condnet_w;
+    const size_t cnt[8] = {576, 64, 4096, 64, 4096, 64, 2048, 32};
+    for (int q = 0; q < 8; ++q) { cudaMemcpyAsync(dd, pw[q], cnt[q] * 4, cudaMemcpyDeviceToDevice, s); dd += cnt[q]; }
+    st = sr_alloc(n, (void**)&n->condnet_mma, (size_t)cnm_layout().total);
+    if (st) return st;
+    K4_CUDA_TRY(cudaMemsetAsync(n->condnet_mma, 0, cnm_layout().total, s));
+    pack_condnet_mma_kernel<<<16, 256, 0, s>>>(n->condnet_w, n->condnet_mma);
     K4_CUDA_TRY(cudaGetLastError());
     return K4_OK;
 }
@@ -1366,13 +1384,46 @@ int launch_sft_mma(const SftParams& p, const unsigned char* frag, cudaStream_t s
     return K4_OK;
 }
 
-int run_sft(const SrSft& f, SftParams p, cudaStream_t s) {
+// Which kernel runs a CondNet or standalone SFT pass (the K4_SR_KERNEL_* values of k4_testing_condnet / k4_testing_sft).
+// SRP_AUTO is the decoder's own choice, env switch included; both kernels run every shape, so a forced one always runs.
+enum SrPixelKernel { SRP_AUTO = 0, SRP_MMA = 1, SRP_FP32 = 2 };
+
+// sel: SrPixelKernel; *used (if given) receives the kernel that ran.
+int run_sft(const SrSft& f, SftParams p, cudaStream_t s, int sel = SRP_AUTO, int* used = nullptr) {
     static const bool use_fp32 = getenv("K4_SFT_FP32") != nullptr;      // development switch: fp32 FFMA kernel
-    if (use_fp32) {
+    const bool fp32 = (sel == SRP_AUTO) ? use_fp32 : sel == SRP_FP32;
+    if (used) *used = fp32 ? SRP_FP32 : SRP_MMA;
+    if (fp32) {
         p.w = f.w;
         return f.cout == 64 ? launch_sft<64>(p, s) : launch_sft<32>(p, s);
     }
     return f.cout == 64 ? launch_sft_mma<64>(p, f.frag, s) : launch_sft_mma<32>(p, f.frag, s);
+}
+
+// CondNet on rows [y_lo, y_hi) of an h x w condition map: cond32 (fp32 [h*w][32]) and, if given, cond16 (the fp16 operand
+// of the fused SFT epilogues) of those rows.  AUTO reads K4_CONDNET_FP32 per call (fp32 FFMA kernel when it is "1").
+int run_condnet(const k4_srnet* n, const float* cond_in, int h, int w, int y_lo, int y_hi, float* cond32, __half* cond16,
+                cudaStream_t s, int sel = SRP_AUTO, int* used = nullptr) {
+    bool fp32 = sel == SRP_FP32;
+    if (sel == SRP_AUTO) { const char* cenv = getenv("K4_CONDNET_FP32"); fp32 = cenv && cenv[0] == '1'; }
+    if (fp32) {
+        CondParams cp{cond_in, n->condnet_w, cond32, h, w, y_lo, y_hi, cond16};
+        constexpr int NW = 64 * 9 + 64 + 2 * (64 * 64 + 64) + 32 * 64 + 32;
+        if (int st = sr_set_smem(condnet_kernel, 11, NW * 4)) return st;
+        const long long np = (long long)(y_hi - y_lo) * w;
+        K4_CUDA_TRY(sr_launch(condnet_kernel, (unsigned)((np + 127) / 128), 128, (size_t)NW * 4, s, cp));
+    } else {
+        CondMmaParams cp{cond_in, n->condnet_mma, cond32, cond16, h, w, y_lo, y_hi};
+        const int smem = cnm_layout().total;
+        if (int st = sr_set_smem(condnet_mma_kernel, 12, smem)) return st;
+        const long long nb = ((long long)(y_hi - y_lo) * w + 15) / 16;
+        long long grid = (nb + 3) / 4;
+        const long long cap = (long long)sr_dev()->sms * 4;
+        if (grid > cap) grid = cap;
+        K4_CUDA_TRY(sr_launch(condnet_mma_kernel, (unsigned)(grid < 1 ? 1 : grid), 128, (size_t)smem, s, cp));
+    }
+    if (used) *used = fp32 ? SRP_FP32 : SRP_MMA;
+    return K4_OK;
 }
 
 }  // namespace
@@ -1404,18 +1455,7 @@ extern "C" int k4_srnet_create(const k4_srnet_desc* d, k4_stream_t stream, k4_sr
     int k = 0;
 #define SR_TRY(x) do { st = (x); if (st != K4_OK) { k4_srnet_destroy(n); return st; } } while (0)
     SR_TRY(make_conv(n, n->conv_first, P[k], P[k + 1], 64, 3, s)); k += 2;
-    {   // CondNet.0 (64x1x3x3), .2 (64x64), .4 (64x64), .6 (32x64)
-        const size_t nw = 64 * 9 + 64 + 2 * (64 * 64 + 64) + 32 * 64 + 32;
-        SR_TRY(sr_alloc(n, (void**)&n->condnet_w, nw * 4));
-        float* dd = n->condnet_w;
-        const size_t cnt[8] = {576, 64, 4096, 64, 4096, 64, 2048, 32};
-        for (int q = 0; q < 8; ++q) { cudaMemcpyAsync(dd, P[k + q], cnt[q] * 4, cudaMemcpyDeviceToDevice, s); dd += cnt[q]; }
-        k += 8;
-        SR_TRY(sr_alloc(n, (void**)&n->condnet_mma, (size_t)cnm_layout().total));
-        K4_CUDA_TRY(cudaMemsetAsync(n->condnet_mma, 0, cnm_layout().total, s));
-        pack_condnet_mma_kernel<<<16, 256, 0, s>>>(n->condnet_w, n->condnet_mma);
-        K4_CUDA_TRY(cudaGetLastError());
-    }
+    SR_TRY(make_condnet(n, P + k, s)); k += 8;
     for (int i = 0; i < d->num_block; ++i) {
         for (int j = 0; j < 3; ++j) {
             for (int c = 0; c < 5; ++c) {
@@ -1498,23 +1538,7 @@ static int srnet_forward_roi_impl(const k4_srnet* n, const float* d_x, const flo
     K4_CUDA_TRY(sr_launch(nchw_to_nhwc32_kernel, (unsigned)((P * 32 + 255) / 256), 256, 0, s, d_x, in16, 3, P));
     {
         const SrRows rr = sr_rows(ky0, ky1, 3 + 5 * nrdb + 5, h);          // every SFT layer inside the window reads it
-        const char* cenv = getenv("K4_CONDNET_FP32");
-        if (cenv && cenv[0] == '1') {
-            CondParams cp{d_cond, n->condnet_w, cond32, h, w, rr.lo, rr.hi, fuse ? cond16 : nullptr};
-            constexpr int NW = 64 * 9 + 64 + 2 * (64 * 64 + 64) + 32 * 64 + 32;
-            SR_DO(sr_set_smem(condnet_kernel, 11, NW * 4));
-            const long long np = (long long)(rr.hi - rr.lo) * w;
-            K4_CUDA_TRY(sr_launch(condnet_kernel, (unsigned)((np + 127) / 128), 128, (size_t)NW * 4, s, cp));
-        } else {
-            CondMmaParams cp{d_cond, n->condnet_mma, cond32, fuse ? cond16 : nullptr, h, w, rr.lo, rr.hi};
-            const int smem = cnm_layout().total;
-            SR_DO(sr_set_smem(condnet_mma_kernel, 12, smem));
-            const long long nb = ((long long)(rr.hi - rr.lo) * w + 15) / 16;
-            long long grid = (nb + 3) / 4;
-            const long long cap = (long long)sr_dev()->sms * 4;
-            if (grid > cap) grid = cap;
-            K4_CUDA_TRY(sr_launch(condnet_mma_kernel, (unsigned)(grid < 1 ? 1 : grid), 128, (size_t)smem, s, cp));
-        }
+        SR_DO(run_condnet(n, d_cond, h, w, rr.lo, rr.hi, cond32, fuse ? cond16 : nullptr, s));
     }
     ConvParams c0{};
     c0.H = h; c0.W = w;
@@ -1736,6 +1760,74 @@ extern "C" int k4_testing_conv3x3(const k4_conv_test_args* a, int32_t* kernel_us
     }
     const cudaError_t e = cudaStreamSynchronize(s);       // the packs are freed below
     if (st == K4_OK && e != cudaSuccess) { k4_set_cuda_error(e, "k4_testing_conv3x3"); st = K4_ERR_CUDA; }
+    k4_srnet_destroy(n);
+    if (st == K4_OK && kernel_used) *kernel_used = used;
+    return st;
+}
+
+// CondNet for the test suite: a throw-away k4_srnet holds the packs (make_condnet, as k4_srnet_create builds them),
+// run_condnet runs them with the requested kernel and the decoder's grid, k4_srnet_destroy frees them.
+extern "C" int k4_testing_condnet(const k4_condnet_test_args* a, int32_t* kernel_used, k4_stream_t stream) {
+    if (kernel_used) *kernel_used = -1;
+    if (!a || !a->h_condnet || !a->d_cond_in || !a->d_cond_out) return K4_ERR_INVALID_ARG;
+    for (int i = 0; i < 8; ++i) if (!a->h_condnet[i]) return K4_ERR_INVALID_ARG;
+    if (a->H < 1 || a->W < 1 || (long long)a->H * a->W > (1LL << 30)) return K4_ERR_INVALID_ARG;
+    if (a->y_lo < 0 || a->y_lo >= a->y_hi || a->y_hi > a->H) return K4_ERR_INVALID_ARG;
+    if (a->kernel < SRP_AUTO || a->kernel > SRP_FP32) return K4_ERR_INVALID_ARG;
+    if (((uintptr_t)a->d_cond_in & 3) || ((uintptr_t)a->d_cond_out & 7) || ((uintptr_t)a->d_cond16 & 3)) return K4_ERR_INVALID_ARG;
+    int st = k4_device_check();
+    if (st != K4_OK) return st;
+
+    cudaStream_t s = (cudaStream_t)stream;
+    k4_srnet* n = new (std::nothrow) k4_srnet();
+    if (!n) return K4_ERR_INVALID_ARG;
+    memset(n, 0, sizeof(*n));
+    int used = -1;
+    st = make_condnet(n, a->h_condnet, s);
+    if (!st) st = run_condnet(n, a->d_cond_in, a->H, a->W, a->y_lo, a->y_hi, a->d_cond_out, static_cast<__half*>(a->d_cond16), s,
+                              a->kernel, &used);
+    const cudaError_t e = cudaStreamSynchronize(s);       // the packs are freed below
+    if (st == K4_OK && e != cudaSuccess) { k4_set_cuda_error(e, "k4_testing_condnet"); st = K4_ERR_CUDA; }
+    k4_srnet_destroy(n);
+    if (st == K4_OK && kernel_used) *kernel_used = used;
+    return st;
+}
+
+// One SFT layer as its own pass for the test suite: make_sft packs it as k4_srnet_create does, run_sft runs it.
+extern "C" int k4_testing_sft(const k4_sft_test_args* a, int32_t* kernel_used, k4_stream_t stream) {
+    if (kernel_used) *kernel_used = -1;
+    if (!a || !a->h_sft || !a->d_cond) return K4_ERR_INVALID_ARG;
+    for (int i = 0; i < 8; ++i) if (!a->h_sft[i]) return K4_ERR_INVALID_ARG;
+    if (a->cout != 32 && a->cout != 64) return K4_ERR_INVALID_ARG;
+    if (a->kernel < SRP_AUTO || a->kernel > SRP_FP32) return K4_ERR_INVALID_ARG;
+    if (a->p0 < 0 || a->P < 1 || a->P > (1LL << 30)) return K4_ERR_INVALID_ARG;
+    if (!a->d_x_f == !a->d_x_h || !a->d_dst_h == !a->d_dst_f) return K4_ERR_INVALID_ARG;       // exactly one input, one output
+    if (a->d_x_h && (a->xh_c0 < 0 || a->xh_c0 % 2 || a->xh_cstride % 2 || a->xh_c0 + a->cout > a->xh_cstride)) return K4_ERR_INVALID_ARG;
+    if (a->d_dst_h && (a->dst_c0 < 0 || a->dst_c0 % 8 || a->dst_cstride % 8 || a->dst_c0 + a->cout > a->dst_cstride)) return K4_ERR_INVALID_ARG;
+    if (a->d_dst_f && !a->d_res_f) return K4_ERR_INVALID_ARG;
+    if (((uintptr_t)a->d_cond & 15) || ((uintptr_t)a->d_x_f & 7) || ((uintptr_t)a->d_x_h & 3) || ((uintptr_t)a->d_dst_h & 15) ||
+        ((uintptr_t)a->d_dst_f & 7) || ((uintptr_t)a->d_res_f & 7))
+        return K4_ERR_INVALID_ARG;
+    int st = k4_device_check();
+    if (st != K4_OK) return st;
+
+    cudaStream_t s = (cudaStream_t)stream;
+    k4_srnet* n = new (std::nothrow) k4_srnet();
+    if (!n) return K4_ERR_INVALID_ARG;
+    memset(n, 0, sizeof(*n));
+    int used = -1;
+    st = make_sft(n, n->sftbody, a->h_sft, a->cout, s);
+    if (!st) {
+        SftParams p{};
+        p.cond = a->d_cond;
+        p.x_f = a->d_x_f; p.x_h = static_cast<const __half*>(a->d_x_h); p.xh_cstride = a->xh_cstride; p.xh_c0 = a->xh_c0;
+        p.dst_h = static_cast<__half*>(a->d_dst_h); p.dst_cstride = a->dst_cstride; p.dst_c0 = a->dst_c0;
+        p.dst_f = a->d_dst_f; p.res_f = a->d_res_f; p.res_scale = a->res_scale;
+        p.p0 = a->p0; p.P = a->P;
+        st = run_sft(n->sftbody, p, s, a->kernel, &used);
+    }
+    const cudaError_t e = cudaStreamSynchronize(s);       // the packs are freed below
+    if (st == K4_OK && e != cudaSuccess) { k4_set_cuda_error(e, "k4_testing_sft"); st = K4_ERR_CUDA; }
     k4_srnet_destroy(n);
     if (st == K4_OK && kernel_used) *kernel_used = used;
     return st;

@@ -81,6 +81,29 @@ class ConvTestArgs(C.Structure):
     ]
 
 
+K4_SR_KERNEL_AUTO, K4_SR_KERNEL_MMA, K4_SR_KERNEL_FP32 = 0, 1, 2
+
+
+class CondnetTestArgs(C.Structure):
+    """k4_condnet_test_args: CondNet on a row window for the test suite (k4_testing_condnet)."""
+    _fields_ = [
+        ('h_condnet', C.POINTER(C.c_void_p)), ('d_cond_in', C.c_void_p), ('H', C.c_int32), ('W', C.c_int32),
+        ('y_lo', C.c_int32), ('y_hi', C.c_int32), ('d_cond_out', C.c_void_p), ('d_cond16', C.c_void_p),
+        ('kernel', C.c_int32), ('reserved0', C.c_int32),
+    ]
+
+
+class SftTestArgs(C.Structure):
+    """k4_sft_test_args: one SFT layer as its own pass for the test suite (k4_testing_sft)."""
+    _fields_ = [
+        ('h_sft', C.POINTER(C.c_void_p)), ('cout', C.c_int32), ('kernel', C.c_int32), ('d_cond', C.c_void_p),
+        ('d_x_f', C.c_void_p), ('d_x_h', C.c_void_p), ('xh_cstride', C.c_int32), ('xh_c0', C.c_int32),
+        ('d_dst_h', C.c_void_p), ('dst_cstride', C.c_int32), ('dst_c0', C.c_int32),
+        ('d_dst_f', C.c_void_p), ('d_res_f', C.c_void_p), ('res_scale', C.c_float), ('reserved0', C.c_int32),
+        ('p0', C.c_int64), ('P', C.c_int64),
+    ]
+
+
 # k4_testing_march_phases: counters per warpgroup and their slots (marchers: K4_PH_M_*, MLP groups: K4_PH_L_*)
 K4_PHASE_SLOTS = 8
 MARCHER_PHASES = {1: 'setup', 2: 'march', 3: 'rendezvous', 4: 'wait_done', 5: 'drain', 6: 'store'}
@@ -154,6 +177,8 @@ EXPORTS = {
     'k4_make_rays': (C.c_int, [C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_int32,
                                C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'k4_testing_conv3x3': (C.c_int, [C.POINTER(ConvTestArgs), C.POINTER(C.c_int32), C.c_void_p]),
+    'k4_testing_condnet': (C.c_int, [C.POINTER(CondnetTestArgs), C.POINTER(C.c_int32), C.c_void_p]),
+    'k4_testing_sft': (C.c_int, [C.POINTER(SftTestArgs), C.POINTER(C.c_int32), C.c_void_p]),
     'k4_testing_rgbnet': (C.c_int, [C.c_void_p, C.POINTER(RgbnetTestArgs), C.POINTER(C.c_int32), C.c_void_p]),
     'k4_testing_march_phases': (C.c_int, [C.c_void_p, C.POINTER(RenderArgs), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                           C.POINTER(RenderOut), C.c_void_p, C.c_size_t, C.c_void_p, C.c_int32,

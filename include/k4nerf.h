@@ -417,6 +417,62 @@ typedef struct k4_conv_test_args {
 K4_API int k4_testing_conv3x3(const k4_conv_test_args* args, int32_t* kernel_used, k4_stream_t stream);
 
 /*
+ * k4_testing_condnet / k4_testing_sft: the decoder's per-pixel MLPs -- CondNet and one SFT layer as its own pass -- packed
+ * by the packers k4_srnet_create uses and run by the decoder's own launchers, so that a test can compare them element
+ * by element with a reference.
+ *   kernel: K4_SR_KERNEL_AUTO picks what k4_srnet_forward would (K4_CONDNET_FP32, read per call; K4_SFT_FP32, latched at
+ *   the first SFT pass of a process); MMA / FP32 force condnet_mma_kernel / sft_mma_kernel or condnet_kernel /
+ *   sft_kernel, which run every valid shape.  *kernel_used (may be NULL) receives the kernel that ran, -1 on error.
+ *   Arguments are checked before any CUDA call (K4_ERR_INVALID_ARG).  The calls synchronise `stream`.
+ *
+ * k4_testing_condnet: CondNet (conv3x3 1 -> 64, LeakyReLU 0.2, 1x1 64 -> 64, LeakyReLU, 1x1 64 -> 64, LeakyReLU,
+ * 1x1 64 -> 32) on rows [y_lo, y_hi) of an H x W condition map, zero padded at the map's border.
+ *   h_condnet: HOST array of the 8 device pointers in k4_srnet_desc order (CondNet.0 w [64][1][3][3], b [64], .2 w
+ *   [64][64], b, .4 w [64][64], b, .6 w [32][64], b [32]).  d_cond_in fp32 [H][W].  d_cond_out fp32 [H*W][32] and d_cond16
+ *   (fp16 [H*W][32], the operand of the fused SFT epilogues, NULL to skip) receive the window's rows only.
+ *
+ * k4_testing_sft: one SFT layer, y = x * (scale + 1) + shift, on pixels [p0, p0 + P) of per-pixel buffers.
+ *   h_sft: HOST array of the layer's 8 device pointers (the h_sft convention of k4_conv_test_args); cout 32 or 64.
+ *   d_cond fp32 [..][32].  Input: d_x_f (fp32 [..][64], channels [0, cout)) or d_x_h (fp16, channels [xh_c0, xh_c0 +
+ *   cout) of xh_cstride, both even), not both.  Output: d_dst_h (fp16, channels [dst_c0, dst_c0 + cout) of dst_cstride,
+ *   both multiples of 8; may be d_x_h) or d_dst_f (fp32 [..][64]) = y * res_scale + d_res_f, where d_res_f may equal
+ *   d_dst_f (the RRDB tail), not both.
+ */
+enum { K4_SR_KERNEL_AUTO = 0,              /* the decoder's own choice                           */
+       K4_SR_KERNEL_MMA = 1,               /* condnet_mma_kernel / sft_mma_kernel (mma.sync)     */
+       K4_SR_KERNEL_FP32 = 2 };            /* condnet_kernel / sft_kernel (fp32 FFMA)            */
+
+typedef struct k4_condnet_test_args {
+    const float* const* h_condnet;
+    const float* d_cond_in;
+    int32_t H, W;
+    int32_t y_lo, y_hi;
+    float* d_cond_out;
+    void* d_cond16;                        /* fp16, or NULL */
+    int32_t kernel;
+    int32_t reserved0;
+} k4_condnet_test_args;
+K4_API int k4_testing_condnet(const k4_condnet_test_args* args, int32_t* kernel_used, k4_stream_t stream);
+
+typedef struct k4_sft_test_args {
+    const float* const* h_sft;
+    int32_t cout;
+    int32_t kernel;
+    const float* d_cond;
+    const float* d_x_f;
+    const void* d_x_h;                     /* fp16 */
+    int32_t xh_cstride, xh_c0;
+    void* d_dst_h;                         /* fp16 */
+    int32_t dst_cstride, dst_c0;
+    float* d_dst_f;
+    const float* d_res_f;
+    float res_scale;
+    int32_t reserved0;
+    int64_t p0, P;
+} k4_sft_test_args;
+K4_API int k4_testing_sft(const k4_sft_test_args* args, int32_t* kernel_used, k4_stream_t stream);
+
+/*
  * k4_testing_rgbnet: the scene's packed rgbnet on rows the caller supplies, run by the marchers' own device code for one
  * K4_MLP_* mode, so that a test can compare the colour MLP sample by sample with a reference.
  *   d_x [n][dim0]: model-layout MLP inputs, the vectors the reference's rgbnet receives (rgb_feat: the k0 channels fed to

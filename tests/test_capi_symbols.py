@@ -96,6 +96,76 @@ def test_testing_conv3x3_validates_arguments_without_a_gpu():
     assert lib.k4_testing_conv3x3(C.byref(args(upsample2x=1, **sft)), C.byref(used), None) == -2
 
 
+def test_testing_condnet_validates_arguments_without_a_gpu():
+    """k4_testing_condnet (CondNet on a row window for the GPU tests): bad arguments are reported as K4_ERR_INVALID_ARG
+    before any CUDA call, and *kernel_used says that nothing ran."""
+    from k4nerf import _lib
+    C = ctypes
+    lib = _lib.lib
+    A = _lib.CondnetTestArgs
+    assert C.sizeof(A) == 56 and A.H.offset == 16 and A.d_cond_out.offset == 32 and A.kernel.offset == 48   # the header's layout
+    buf = C.create_string_buffer(64)
+    ptrs = (C.c_void_p * 8)(*([C.addressof(buf)] * 8))
+    holey = (C.c_void_p * 8)(*([C.addressof(buf)] * 7 + [None]))
+
+    def args(**kw):
+        a = A()
+        a.h_condnet = C.cast(ptrs, C.POINTER(C.c_void_p))
+        a.d_cond_in = a.d_cond_out = a.d_cond16 = C.addressof(buf)
+        a.H, a.W, a.y_lo, a.y_hi = 8, 8, 0, 8
+        for k, v in kw.items():
+            setattr(a, k, v)
+        return a
+
+    used = C.c_int32(7)
+    bad = [dict(h_condnet=None), dict(h_condnet=C.cast(holey, C.POINTER(C.c_void_p))), dict(d_cond_in=None),
+           dict(d_cond_out=None), dict(H=0), dict(W=0), dict(H=1 << 16, W=1 << 15), dict(y_lo=5, y_hi=4),
+           dict(y_lo=3, y_hi=3), dict(y_hi=9), dict(y_lo=-1), dict(kernel=3), dict(kernel=-1),
+           dict(d_cond_out=C.addressof(buf) + 4), dict(d_cond16=C.addressof(buf) + 2), dict(d_cond_in=C.addressof(buf) + 1)]
+    for kw in bad:
+        used.value = 7
+        assert lib.k4_testing_condnet(C.byref(args(**kw)), C.byref(used), None) == -1, kw
+        assert used.value == -1, kw
+    assert lib.k4_testing_condnet(None, C.byref(used), None) == -1
+
+
+def test_testing_sft_validates_arguments_without_a_gpu():
+    """k4_testing_sft (one SFT layer as its own pass for the GPU tests): bad arguments are reported as K4_ERR_INVALID_ARG
+    before any CUDA call, and *kernel_used says that nothing ran."""
+    from k4nerf import _lib
+    C = ctypes
+    lib = _lib.lib
+    A = _lib.SftTestArgs
+    assert C.sizeof(A) == 104 and A.d_cond.offset == 16 and A.xh_cstride.offset == 40 and A.d_dst_f.offset == 64
+    assert A.res_scale.offset == 80 and A.p0.offset == 88 and A.P.offset == 96                          # the header's layout
+    buf = C.create_string_buffer(64)
+    ptrs = (C.c_void_p * 8)(*([C.addressof(buf)] * 8))
+    holey = (C.c_void_p * 8)(*([None] + [C.addressof(buf)] * 7))
+
+    def args(**kw):
+        a = A()
+        a.h_sft = C.cast(ptrs, C.POINTER(C.c_void_p))
+        a.d_cond = a.d_x_h = a.d_dst_h = C.addressof(buf)
+        a.cout, a.xh_cstride, a.xh_c0, a.dst_cstride, a.dst_c0, a.p0, a.P = 32, 192, 160, 192, 160, 58, 406
+        for k, v in kw.items():
+            setattr(a, k, v)
+        return a
+
+    used = C.c_int32(7)
+    b = C.addressof(buf)
+    bad = [dict(h_sft=None), dict(h_sft=C.cast(holey, C.POINTER(C.c_void_p))), dict(d_cond=None), dict(cout=16),
+           dict(cout=48), dict(kernel=3), dict(kernel=-1), dict(p0=-1), dict(P=0), dict(P=(1 << 30) + 1),
+           dict(d_x_h=None), dict(d_x_f=b), dict(d_dst_h=None), dict(d_dst_f=b, d_res_f=b),
+           dict(d_dst_h=None, d_dst_f=b), dict(xh_c0=161), dict(xh_cstride=191), dict(xh_c0=-2), dict(cout=64),
+           dict(dst_c0=164), dict(dst_cstride=196), dict(d_cond=b + 8), dict(d_x_h=b + 2), dict(d_dst_h=b + 8),
+           dict(d_dst_h=None, d_dst_f=b + 4, d_res_f=b), dict(d_dst_h=None, d_dst_f=b, d_res_f=b + 4)]
+    for kw in bad:
+        used.value = 7
+        assert lib.k4_testing_sft(C.byref(args(**kw)), C.byref(used), None) == -1, kw
+        assert used.value == -1, kw
+    assert lib.k4_testing_sft(None, C.byref(used), None) == -1
+
+
 def test_testing_rgbnet_validates_arguments_without_a_gpu():
     """k4_testing_rgbnet (a scene's rgbnet on caller rows for the GPU tests): bad arguments are reported as
     K4_ERR_INVALID_ARG before any CUDA call, and *group_rows stays 0.  The scene here is a zero-filled host block: a scene

@@ -176,7 +176,8 @@ def test_pretrained_full_frame_tile_process_vs_cudnn_fp32(net_pretrained, cuda_d
 
 def test_large_magnitude_activations_do_not_overflow_fp16(cuda_device):
     """Conv / SFT operands are fp16: weights scaled so that the trunk reaches ~1e3 and the SFT modulation
-    multiplies it further.  Every fp32 -> fp16 conversion in the kernels saturates (cvt.rn.satfinite), so no
+    multiplies it further.  Every fp32 -> fp16 conversion of a computed activation or condition in the kernels
+    saturates (cvt.rn.satfinite; CondNet's hi + lo split and its fp16 condition included), so no
     inf/nan may appear and the result must stay close to the fp32 network wherever the fp32 network's own
     intermediate values are representable."""
     sd = sftnet.random_state_dict(seed=5, scale=1.0)

@@ -7,8 +7,9 @@ upsampling for the up layers), followed by the epilogue written out in torch and
 in float64.
 
 (a) exact operands: torch.equal against the reference; (b) random operands: the precision contract of DESIGN.md,
-element by element; (c) the fused SFT epilogues; and, in child interpreters, the whole network under each of the
-decoder's A/B environment switches.
+element by element; (c) the fused SFT epilogues; (d) CondNet, both kernels (k4_testing_condnet); (e) the standalone
+SFT pass, both kernels, in the decoder's four I/O forms (k4_testing_sft); (f) the fp16 saturation of the condition;
+and, in child interpreters, the whole network under each of the decoder's A/B environment switches.
 """
 import ctypes as C
 import math
@@ -659,6 +660,397 @@ def test_sft_epilogues(case, kernel, cuda_device):
     if kernel == AUTO:
         ws = WS_CP if os.environ.get('K4_CONV_NO_TMA', '0')[:1] == '1' else WS_TMA
         assert used == ws
+
+
+# ------------------------------------------------------------------------------------------------
+# (d) CondNet
+# ------------------------------------------------------------------------------------------------
+MMA, FP32 = _lib.K4_SR_KERNEL_MMA, _lib.K4_SR_KERNEL_FP32
+PKNAME = {_lib.K4_SR_KERNEL_AUTO: 'auto', MMA: 'mma', FP32: 'fp32'}
+U = 2.0 ** -24                   # unit roundoff of fp32
+GAMMA_TC = 17 * 2.0 ** -23       # one mma.sync instruction, relative to S (test_gpu_march_mlp.py)
+
+
+def _stream():
+    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def condnet_params(seed, dev, scale=1.0):
+    """CondNet.0 (64x1x3x3), .2, .4 (64x64x1x1), .6 (32x64x1x1), weight and bias each, as nn.Conv2d initialises them
+    (uniform in +-1 / sqrt(fan_in)), times `scale`."""
+    g = torch.Generator().manual_seed(seed)
+    ts = []
+    for shape, fan in (((64, 1, 3, 3), 9), ((64, 64, 1, 1), 64), ((64, 64, 1, 1), 64), ((32, 64, 1, 1), 64)):
+        bound = scale / math.sqrt(fan)
+        ts += [(torch.rand(shape, generator=g) * 2 - 1) * bound, (torch.rand(shape[0], generator=g) * 2 - 1) * bound]
+    return [t.contiguous().to(dev) for t in ts]
+
+
+def depth_map(H, W, seed, dev):
+    """A depth-like condition in [0, 1]: a ramp, flat plateaus with sharp edges, a noisy patch, exact 0 and 1 flats."""
+    g = torch.Generator().manual_seed(seed)
+    y, x = torch.linspace(0, 1, H)[:, None], torch.linspace(0, 1, W)[None]
+    d = (0.3 + 0.5 * x * (1 - 0.5 * y)).expand(H, W).clone()
+    for _ in range(4):
+        y0, x0 = int(torch.randint(0, H, (1,), generator=g)), int(torch.randint(0, W, (1,), generator=g))
+        d[y0:y0 + max(1, H // 3), x0:x0 + max(1, W // 3)] = torch.rand(1, generator=g).item()
+    d[H // 2:, W // 2:W // 2 + max(1, W // 4)] = torch.rand(H - H // 2, min(W, W // 2 + max(1, W // 4)) - W // 2, generator=g)
+    d[:max(1, H // 5)] = 1.0
+    d[:, :W // 6] = 0.0
+    return d.clamp(0, 1).contiguous().to(dev)
+
+
+def run_condnet(params, cond_in, kernel, rows=None):
+    """One k4_testing_condnet call into sentinel-filled cond_out [P, 32] / cond16 [P, 32].  Returns them and the kernel."""
+    H, W = cond_in.shape
+    out = torch.full((H * W, 32), SENT32, device=cond_in.device)
+    c16 = torch.full((H * W, 32), SENT16, dtype=torch.float16, device=cond_in.device)
+    a = _lib.CondnetTestArgs()
+    a.h_condnet = _sft_ptrs(params)
+    a.d_cond_in, a.H, a.W = cond_in.data_ptr(), H, W
+    a.y_lo, a.y_hi = rows if rows is not None else (0, H)
+    a.d_cond_out, a.d_cond16, a.kernel = out.data_ptr(), c16.data_ptr(), kernel
+    used = C.c_int32(-9)
+    st = _lib.lib.k4_testing_condnet(C.byref(a), C.byref(used), _stream())
+    assert st == OK, f'k4_testing_condnet -> {st} ({_lib.lib.k4_status_string(st).decode()}) for {PKNAME[kernel]}'
+    if kernel != _lib.K4_SR_KERNEL_AUTO:
+        assert used.value == kernel, (PKNAME[kernel], used.value)
+    return out, c16, used.value
+
+
+def lrelu(t):
+    return torch.where(t > 0, t, 0.2 * t)
+
+
+def condnet_ref(p, cond_in, kernel):
+    """fp64 CondNet on the whole map: conv3x3 with zero padding, then the three 1x1 layers, LeakyReLU 0.2 between.
+    Returns the output [P, 32], the per-element bound E of `kernel` [P, 32] and the largest |hidden activation|.
+
+    The bound is carried layer to layer: e_{l+1} = gamma_l * S_{l+1} + |W_{l+1}| e_l, S = |b| + sum |a| |w| over the
+    layer's products, with |a| taken as |a_ref| + e_l.  LeakyReLU is 1-Lipschitz; its fp32 multiply by 0.2f (not 0.2)
+    adds at most 2u |z|.  u = 2^-24.
+      * Layer 0 (both kernels): an FFMA chain of 9 products from the bias, 10u * S.
+      * fp32 kernel, 1x1 layers: an FFMA chain of 64 products, 65u * S.
+      * mma kernel, 1x1 layers: x = hi + lo with hi = fp16(x), lo = fp16(x - hi) for activations and weights alike:
+        |x - hi - lo| <= 2^-22 |x| + 2^-25 (a lo part below 2^-14 is an fp16 subnormal, spaced 2^-24 -- the case of
+        |x| < 2^-3, so of most 1x1 weights, bound 1/8) and |lo| <= 2^-11 |x| + 2^-24.  The product drops lo_a lo_w and
+        the two representation errors; its S counts the three fp16 products.  Four k16 steps of three MMAs are 12
+        instructions, each within 17 * 2^-23 * S (a truncating fp32 accumulation of 16 exact products, the model of
+        test_gpu_march_mlp.py): 12 * 17 * 2^-23 * S, about 2^-15.3 S.
+    Carried through |W| (sum |w| is about 4 per row at nn.Conv2d initialisation) the output bound of default weights
+    ends near 2^-10 of the output scale: it catches a wrong tap, padding row, window or layer, but not a lost lo term of
+    random sign (about 2^-15 S); test_condnet_exact_operands checks the lo terms bit for bit."""
+    W0, b0 = p[0].double(), p[1].double()
+    c = cond_in.double()[None, None]
+    z = hwc(F.conv2d(c, W0, b0, padding=1)[0])
+    E = 10 * U * (hwc(F.conv2d(c.abs(), W0.abs(), padding=1)[0]) + b0.abs())
+    hmax = 0.0
+    for i in (2, 4, 6):
+        a = lrelu(z)
+        D = E + 2 * U * (z.abs() + E)
+        hmax = max(hmax, a.abs().max().item())
+        Wl, bl = p[i].double().view(p[i].shape[0], 64), p[i + 1].double()
+        av, aw = a.abs() + D, Wl.abs()
+        z = a @ Wl.T + bl
+        if kernel == FP32:
+            E = D @ aw.T + 65 * U * (av @ aw.T + bl.abs())
+        else:
+            ev, lv = 2.0 ** -22 * av + 2.0 ** -25, 2.0 ** -11 * av + 2.0 ** -24
+            ew, lw = 2.0 ** -22 * aw + 2.0 ** -25, 2.0 ** -11 * aw + 2.0 ** -24
+            split = lv @ lw.T + av @ ew.T + ev @ aw.T + ev @ ew.T
+            S = av @ aw.T + av @ lw.T + lv @ aw.T + bl.abs()
+            E = D @ aw.T + split + 12 * GAMMA_TC * S
+    return z, E, hmax
+
+
+def check_condnet_outputs(out, c16, ref, bound, rows, H, W, label):
+    """cond_out within the bound (or equal to ref when bound is None) on the window's rows; cond16 is bitwise the saturated
+    fp16 rounding of the kernel's own cond_out; every row outside the window keeps its sentinel."""
+    ylo, yhi = rows if rows is not None else (0, H)
+    win = slice(ylo * W, yhi * W)
+    got = out[win]
+    if bound is None:
+        check_exact([('cond_out', got, ref[win].float(), None)])
+        worst = 0.0
+    else:
+        worst = check_bound([('cond_out', got, ref[win], bound[win])], label)
+    want16 = got.clamp(-FP16_MAX, FP16_MAX).half()
+    assert torch.equal(c16[win].view(torch.int16), want16.view(torch.int16)), 'cond16 is not the saturated fp16 rounding of cond_out'
+    outside = torch.ones(H * W, dtype=torch.bool, device=out.device)
+    outside[win] = False
+    assert bool((out[outside] == SENT32).all()) and bool((c16[outside] == SENT16).all()), 'rows outside the window written'
+    return worst
+
+
+CONDNET_CASES = [  # (name, H, W, rows, weight scale)
+    ('1x1', 1, 1, None, 1.0), ('1x7', 1, 7, None, 1.0), ('7x1', 7, 1, None, 4.0), ('19x13', 19, 13, None, 1.0),
+    ('19x13_w4', 19, 13, None, 4.0), ('rows5-6', 40, 29, (5, 6), 1.0), ('rows3-37', 40, 29, (3, 37), 4.0),
+    ('rows16-33', 40, 29, (16, 33), 1.0),
+]
+
+
+@pytest.mark.parametrize('kernel', (MMA, FP32), ids=PKNAME.get)
+@pytest.mark.parametrize('case', CONDNET_CASES, ids=lambda c: c[0])
+def test_condnet_meets_its_element_bound(case, kernel, cuda_device):
+    """CondNet on depth-like maps (flats, sharp edges, noise) with nn.Conv2d-initialised weights x1 and x4, at shapes
+    down to 1x1, P = 247 (not a multiple of 16) and row windows strictly inside the map, whose edge rows must see the
+    real neighbour rows above and below: every output within the bound of condnet_ref."""
+    name, H, W, rows, scale = case
+    p = condnet_params(70 + H + W, 'cuda', scale)
+    cond_in = depth_map(H, W, 71 + H, 'cuda')
+    ref, E, _ = condnet_ref(p, cond_in, kernel)
+    out, c16, _ = run_condnet(p, cond_in, kernel, rows)
+    torch.cuda.synchronize()
+    check_condnet_outputs(out, c16, ref, E, rows, H, W, f'condnet {name} ({PKNAME[kernel]})')
+
+
+@pytest.mark.parametrize('kernel', (MMA, FP32), ids=PKNAME.get)
+def test_condnet_grid_stride_wraps(kernel, cuda_device):
+    """More than 3 x (4 * SM-count CTAs x 64 pixels): the mma kernel's capped grid strides over the map more than three
+    times (the fp32 kernel takes one thread per pixel)."""
+    W = 331
+    H = 3 * 4 * sm_count() * 64 // W + 3
+    assert H * W > 3 * 4 * sm_count() * 64
+    p = condnet_params(80, 'cuda')
+    cond_in = depth_map(H, W, 81, 'cuda')
+    ref, E, _ = condnet_ref(p, cond_in, kernel)
+    out, c16, _ = run_condnet(p, cond_in, kernel, (1, H))
+    torch.cuda.synchronize()
+    check_condnet_outputs(out, c16, ref, E, (1, H), H, W, f'condnet {H}x{W} ({PKNAME[kernel]})')
+
+
+def exact_condnet_params(seed, dev):
+    """Non-negative dyadic CondNet weights for test_condnet_exact_operands: W0 j/8 (j <= 2), 1x1 rows of two non-zero
+    weights -- CondNet.2 of 12 significant bits, (2^11 + odd) * 2^-15, so each has an fp16 lo part; CondNet.4 and .6
+    exactly 1/2 -- and biases m/64 (m <= 16)."""
+    g = torch.Generator().manual_seed(seed)
+
+    def sparse(n_out, value):
+        w = torch.zeros(n_out, 64)
+        for o in range(n_out):
+            w[o, torch.randperm(64, generator=g)[:2]] = value(2)
+        return w.view(n_out, 64, 1, 1)
+
+    bias = lambda n: torch.randint(0, 17, (n,), generator=g) / 64.0
+    ts = [torch.randint(0, 3, (64, 1, 3, 3), generator=g) / 8.0, bias(64),
+          sparse(64, lambda n: (2 ** 11 + 2 * torch.randint(0, 2 ** 10, (n,), generator=g) + 1) * 2.0 ** -15), bias(64),
+          sparse(64, lambda n: torch.full((n,), 0.5)), bias(64),
+          sparse(32, lambda n: torch.full((n,), 0.5)), bias(32)]
+    return [t.contiguous().to(dev) for t in ts]
+
+
+@pytest.mark.parametrize('kernel', (MMA, FP32), ids=PKNAME.get)
+def test_condnet_exact_operands(kernel, cuda_device):
+    """Operands whose every sum is exact in fp32 and whose activations fit the mma kernel's 22-bit hi + lo split exactly:
+    the condition on the 1/2 grid, so layer 0's outputs lie on the 2^-4 grid below 2.75 (7 bits, no lo part); CondNet.2
+    weights with lo parts make layer 1's outputs 19-bit values (2^-19 grid, < 1), and the halving 1x1 layers keep 20 and
+    21 bits.  Every lo x lo product is zero (layer 1: no activation lo parts; layers 2, 3: no weight lo parts), so both
+    kernels must EQUAL the fp64 reference: a lost al * Wh term (layers 2, 3), a lost weight lo part (layer 1), a moved
+    tap or a wrong padding row is a non-zero difference."""
+    H, W = 23, 37
+    p = exact_condnet_params(85, 'cuda')
+    cond_in = ((depth_map(H, W, 86, 'cuda') * 2).round() / 2).contiguous()
+    ref, _, _ = condnet_ref(p, cond_in, kernel)
+    # the case's premises, checked on the reference's activations
+    z = hwc(F.conv2d(cond_in.double()[None, None], p[0].double(), p[1].double(), padding=1)[0])
+    for i in (2, 4, 6):
+        hi = z.half().double()
+        assert torch.equal((z - hi).half().double(), z - hi), 'an activation does not fit the hi + lo split'
+        if i > 2:
+            assert bool(((z - hi) != 0).any()), 'no activation lo part: the case lost its point'
+        z = z @ p[i].double().view(-1, 64).T + p[i + 1].double()
+        assert torch.equal(z.float().double(), z)
+    w2 = p[2].view(64, 64)
+    assert bool(((w2 - w2.half().float()) != 0).sum() > 32), 'no weight lo part: the case lost its point'
+    rows = (3, 20)
+    out, c16, _ = run_condnet(p, cond_in, kernel, rows)
+    torch.cuda.synchronize()
+    check_condnet_outputs(out, c16, ref, None, rows, H, W, f'condnet exact ({PKNAME[kernel]})')
+
+
+def test_condnet_auto_follows_the_env_switch_per_call(monkeypatch, cuda_device):
+    """K4_SR_KERNEL_AUTO is the decoder's choice: the mma kernel, or the fp32 kernel while K4_CONDNET_FP32=1 (read per call)."""
+    p = condnet_params(87, 'cuda')
+    cond_in = depth_map(5, 9, 88, 'cuda')
+    monkeypatch.delenv('K4_CONDNET_FP32', raising=False)
+    assert run_condnet(p, cond_in, _lib.K4_SR_KERNEL_AUTO)[2] == MMA
+    monkeypatch.setenv('K4_CONDNET_FP32', '1')
+    assert run_condnet(p, cond_in, _lib.K4_SR_KERNEL_AUTO)[2] == FP32
+
+
+# ------------------------------------------------------------------------------------------------
+# (e) the standalone SFT pass (K4_SR_FUSE_SFT=0, and every decoder call without TMA)
+# ------------------------------------------------------------------------------------------------
+RES_SCALE = float(torch.tensor(0.2, dtype=torch.float32))      # what the kernel multiplies by
+
+
+def run_sft_pass(p, cout, cond, kernel, *, x_f=None, x_h=None, xh_c0=0, dst_h=None, dst_c0=0, dst_f=None, res_f=None,
+                 res_scale=0.0, p0=0, P=1):
+    """One k4_testing_sft call.  x_h / dst_h: fp16 [pixels, cstride]; x_f / dst_f / res_f: fp32 [pixels, 64]."""
+    a = _lib.SftTestArgs()
+    a.h_sft, a.cout, a.kernel, a.d_cond = _sft_ptrs(p), cout, kernel, cond.data_ptr()
+    a.d_x_f, a.d_x_h, a.xh_cstride, a.xh_c0 = _ptr(x_f), _ptr(x_h), (x_h.shape[-1] if x_h is not None else 0), xh_c0
+    a.d_dst_h, a.dst_cstride, a.dst_c0 = _ptr(dst_h), (dst_h.shape[-1] if dst_h is not None else 0), dst_c0
+    a.d_dst_f, a.d_res_f, a.res_scale, a.p0, a.P = _ptr(dst_f), _ptr(res_f), res_scale, p0, P
+    used = C.c_int32(-9)
+    st = _lib.lib.k4_testing_sft(C.byref(a), C.byref(used), _stream())
+    assert st == OK, f'k4_testing_sft -> {st} ({_lib.lib.k4_status_string(st).decode()}) for {PKNAME[kernel]}'
+    if kernel != _lib.K4_SR_KERNEL_AUTO:
+        assert used.value == kernel, (PKNAME[kernel], used.value)
+    return used.value
+
+
+def sft_ref32(p, cond):
+    """fp64 SFT MLPs of one layer on the fp32 condition and fp32 weights, with the fp32 kernel's bounds: FFMA chains of
+    32 products from the bias (33u * S), LeakyReLU's multiply by 0.2f (2u), scale + 1 (u).  Returns sc (scale + 1),
+    e_sc, sh, e_sh like sft_ref."""
+    c = cond.double()
+    W0, b0 = torch.cat([p[0], p[4]]).double(), torch.cat([p[1], p[5]]).double()
+    hid = c @ W0.T + b0
+    e = 33 * U * (c.abs() @ W0.abs().T + b0.abs())
+    a = lrelu(hid)
+    e = e + 2 * U * (hid.abs() + e)
+    out = []
+    for (wi, bi, lo, plus) in ((2, 3, 0, 1.0), (6, 7, 32, 0.0)):
+        W1, b1 = p[wi].double(), p[bi].double()
+        aa, ee = a[:, lo:lo + 32], e[:, lo:lo + 32]
+        y = aa @ W1.T + b1 + plus
+        ey = ee @ W1.abs().T + 33 * U * ((aa.abs() + ee) @ W1.abs().T + b1.abs()) + plus * U * (y.abs() + 1.0)
+        out += [y, ey]
+    return out
+
+
+# (name, what the decoder runs it on): the four I/O forms of run_sft in srnet_forward_roi_impl, each with a row window of
+# a 40 x 29 map as win() gives it
+SFT_FORMS = [('trunk_to_cat', (0, 40)), ('cat_in_place', (13, 27)), ('rrdb_tail_aliased', (14, 26)), ('sbody', (9, 31))]
+
+
+def sft_pass_case(form, cout, kernel, H, W, rows, seed):
+    """Run one form and return [(name, got, ref, bound)] plus the sentinel / untouched checks already asserted."""
+    dev = 'cuda'
+    Pall = H * W
+    p0, P = rows[0] * W, (rows[1] - rows[0]) * W
+    win = slice(p0, p0 + P)
+    g = torch.Generator().manual_seed(seed)
+    p = sft_params(cout, seed + 1, dev)
+    cond = (torch.randn(Pall, 32, generator=g) * 0.5).to(dev)
+    if kernel == FP32:
+        sc, e_sc, sh, e_sh = sft_ref32(p, cond[win])
+    else:
+        sc, e_sc, sh, e_sh = sft_ref(p, cond[win].clamp(-FP16_MAX, FP16_MAX).half())
+    kw = dict(p0=p0, P=P)
+    if form == 'cat_in_place':
+        c0 = 192 - cout
+        buf = (torch.rand(Pall, 192, generator=g) * 3 - 1).half().to(dev)
+        x = buf[win, c0:c0 + cout].double()
+        kw.update(x_h=buf, xh_c0=c0, dst_h=buf, dst_c0=c0)
+    else:
+        xf = trunk_operand(Pall, seed + 2, dev, False)
+        x = xf[win, :cout].double()
+        kw['x_f'] = xf
+    y = x * sc + sh
+    e_y = x.abs() * e_sc + e_sh + FP32_EPS * (y.abs() + (x * sc).abs())
+    if form == 'rrdb_tail_aliased':
+        buf = trunk_operand(Pall, seed + 3, dev, False)
+        c0, cs = 0, 64
+        r = buf[win, :cout].double()
+        kw.update(dst_f=buf, res_f=buf, res_scale=RES_SCALE)
+    elif form != 'cat_in_place':
+        c0, cs = (0, 192) if form == 'trunk_to_cat' else (0, 64)
+        buf = torch.full((Pall, cs), SENT16, dtype=torch.float16, device=dev)
+        kw.update(dst_h=buf, dst_c0=c0)
+    before = buf.clone()
+    used = run_sft_pass(p, cout, cond, kernel, **kw)
+    torch.cuda.synchronize()
+    got = buf[win, c0:c0 + cout].double()
+    if form == 'rrdb_tail_aliased':
+        ref = y * RES_SCALE + r
+        bound = RES_SCALE * e_y + FP32_EPS * ((y * RES_SCALE).abs() + ref.abs())
+    else:
+        ref, bound = y, e_y + 0.5 * ulp16(y.abs() + e_y)
+    keep = torch.ones_like(buf, dtype=torch.bool)
+    keep[win, c0:c0 + cout] = False
+    assert torch.equal(buf[keep].view(torch.int32 if buf.dtype == torch.float32 else torch.int16),
+                       before[keep].view(torch.int32 if buf.dtype == torch.float32 else torch.int16)), \
+        'wrote outside the pixel window / channels'
+    return [(form, got, ref, bound)], used
+
+
+@pytest.mark.parametrize('kernel', (MMA, FP32), ids=PKNAME.get)
+@pytest.mark.parametrize('cout', (32, 64))
+@pytest.mark.parametrize('form', SFT_FORMS, ids=lambda f: f[0])
+def test_sft_pass_meets_its_element_bound(form, cout, kernel, cuda_device):
+    """One SFT layer as its own pass, in each of the decoder's four I/O forms: fp32 trunk in -> fp16 concat channels 0..;
+    fp16 in place at the top channels of the 192-stride concat buffer; fp32 out aliased with the fp32 residual, y * 0.2 +
+    res (the RRDB tail); fp32 trunk in -> the 64-stride sbody.  Pixel windows [p0, p0 + P) with P = 14 * 29, 22 * 29, ...
+    (not multiples of 16).  mma kernel: sft_ref on the saturated fp16 condition (fp16 weights, hidden activation rounded
+    to fp16), carried through x * (scale + 1) + shift and the residual; fp32 kernel: sft_ref32.  fp16 outputs: + half an
+    fp16 ulp of the unrounded value.  Everything outside the window and the layer's channels keeps its bytes."""
+    name, rows = form
+    checks, _ = sft_pass_case(name, cout, kernel, 40, 29, rows, 100 + cout)
+    check_bound(checks, f'sft pass {name} cout {cout} ({PKNAME[kernel]})')
+
+
+@pytest.mark.parametrize('kernel', (MMA, FP32), ids=PKNAME.get)
+@pytest.mark.parametrize('cout', (32, 64))
+def test_sft_pass_grid_stride_wraps(cout, kernel, cuda_device):
+    """More than 3 x (8 * SM-count CTAs x 64 pixels): the mma kernel's capped grid strides over the window more than
+    three times."""
+    W = 331
+    H = 3 * 8 * sm_count() * 64 // W + 4
+    assert (H - 3) * W > 3 * 8 * sm_count() * 64
+    checks, _ = sft_pass_case('rrdb_tail_aliased', cout, kernel, H, W, (2, H - 1), 110 + cout)
+    check_bound(checks, f'sft pass {H}x{W} cout {cout} ({PKNAME[kernel]})')
+
+
+def test_sft_pass_auto_is_the_decoders_choice(cuda_device):
+    """K4_SR_KERNEL_AUTO runs the mma kernel, or the fp32 kernel when the process started with K4_SFT_FP32 set."""
+    _, used = sft_pass_case('sbody', 64, _lib.K4_SR_KERNEL_AUTO, 3, 29, (1, 3), 120)
+    assert used == (FP32 if 'K4_SFT_FP32' in os.environ else MMA)
+
+
+# ------------------------------------------------------------------------------------------------
+# (f) fp16 saturation of the condition
+# ------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize('kernel', (MMA, FP32), ids=PKNAME.get)
+def test_condnet_outputs_beyond_fp16_saturate_cond16(kernel, cuda_device):
+    """CondNet.6 scaled by a power of two (its weights stay below 65504) so that some conditions exceed the fp16 range
+    while every hidden activation stays inside it: cond_out still meets the element bound, cond16 holds +-65504 (the
+    operand the fused SFT epilogues read), and a fused-SFT convolution on that cond16 stays finite."""
+    H, W = 19, 13
+    p = condnet_params(130, 'cuda', 4.0)
+    cond_in = depth_map(H, W, 131, 'cuda')
+    f = 2.0 ** math.floor(math.log2(FP16_MAX / p[6].abs().max().item()))
+    p[6], p[7] = p[6] * f, p[7] * f
+    ref, E, hmax = condnet_ref(p, cond_in, kernel)
+    assert hmax < FP16_MAX and bool((ref > FP16_MAX).any()) and bool((ref < -FP16_MAX).any()), 'the case lost its point'
+    out, c16, _ = run_condnet(p, cond_in, kernel)
+    torch.cuda.synchronize()
+    check_condnet_outputs(out, c16, ref, E, None, H, W, f'condnet saturating ({PKNAME[kernel]})')
+    assert bool((c16 == FP16_MAX).any()) and bool((c16 == -FP16_MAX).any())
+    src, w, b = random_operands(H, W, 64, 64, 64, 132, 'cuda')
+    dst_f = torch.full((H * W, 64), SENT32, device='cuda')
+    dst_h2 = torch.full((H, W, 64), SENT16, dtype=torch.float16, device='cuda')
+    st, used = run_layer(w, b, src, AUTO, mode=6, dst_f=dst_f, dst_h2=dst_h2, cond16=c16, sft=sft_params(64, 133, 'cuda'))
+    expect_ran(st, used, AUTO)
+    torch.cuda.synchronize()
+    assert torch.isfinite(dst_h2).all(), 'the fused SFT epilogue turned a saturated condition into inf / NaN'
+
+
+@pytest.mark.parametrize('kernel', (MMA, FP32), ids=PKNAME.get)
+def test_condnet_hidden_activations_beyond_fp16_stay_finite(kernel, cuda_device):
+    """CondNet.0 scaled by 2^17: layer-0 activations reach about 2e5, beyond fp16 and beyond 65504 + 65504 (so the mma
+    kernel's hi part and its lo part would both overflow without saturation).  Both kernels' outputs stay finite."""
+    H, W = 19, 13
+    p = condnet_params(140, 'cuda')
+    p[0], p[1] = p[0] * 2.0 ** 17, p[1] * 2.0 ** 17
+    cond_in = depth_map(H, W, 141, 'cuda')
+    _, _, hmax = condnet_ref(p, cond_in, kernel)
+    assert hmax > 2 * FP16_MAX, 'the case lost its point'
+    out, c16, _ = run_condnet(p, cond_in, kernel)
+    torch.cuda.synchronize()
+    assert torch.isfinite(out).all() and torch.isfinite(c16).all()
+    assert torch.equal(c16.view(torch.int16), out.clamp(-FP16_MAX, FP16_MAX).half().view(torch.int16))
 
 
 # ------------------------------------------------------------------------------------------------
