@@ -651,6 +651,19 @@ extern "C" int k4_testing_rgbnet(const k4_scene* sc, const k4_rgbnet_test_args* 
     return st;
 }
 
+// ---- the empty-space-skipping field of a scene (test suite) ----
+extern "C" int k4_testing_skip_field(const k4_scene* sc, uint8_t* d_out, int64_t n, int32_t cdims[3]) {
+    if (cdims) cdims[0] = cdims[1] = cdims[2] = 0;
+    if (!sc || !d_out || !cdims || n < 1) return K4_ERR_INVALID_ARG;
+    const K4Dev& v = sc->dev;
+    if (!v.skip) return K4_ERR_UNSUPPORTED;
+    const long long nc = (long long)v.cX * v.cY * v.cZ;
+    if (n < nc) return K4_ERR_INVALID_ARG;
+    K4_CUDA_TRY(cudaMemcpy(d_out, v.skip, (size_t)nc, cudaMemcpyDeviceToDevice));
+    cdims[0] = v.cX; cdims[1] = v.cY; cdims[2] = v.cZ;
+    return K4_OK;
+}
+
 // ---- device memory shared between the ranks of a node (CUDA IPC; one process per GPU) ----
 extern "C" int k4_peer_alloc(size_t bytes, void** d_ptr) {
     if (!d_ptr || bytes == 0) return K4_ERR_INVALID_ARG;

@@ -183,6 +183,7 @@ EXPORTS = {
     'k4_testing_march_phases': (C.c_int, [C.c_void_p, C.POINTER(RenderArgs), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                           C.POINTER(RenderOut), C.c_void_p, C.c_size_t, C.c_void_p, C.c_int32,
                                           C.POINTER(C.c_int32), C.c_void_p]),
+    'k4_testing_skip_field': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int32)]),
 }
 
 if not os.path.exists(LIB_PATH):

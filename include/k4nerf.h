@@ -538,6 +538,20 @@ K4_API int k4_testing_march_phases(const k4_scene* scene, const k4_render_args* 
                                    int64_t n_rays, const k4_render_out* out, void* d_workspace, size_t workspace_bytes,
                                    uint64_t* d_phases, int32_t max_ctas, int32_t* n_ctas, k4_stream_t stream);
 
+/*
+ * k4_testing_skip_field: a copy of the scene's empty-space-skipping field, so that a test can compare it with an
+ * independent distance transform.  The field covers the occupancy mask in cells of 4 x 4 x 4 mask voxels (the last cell
+ * of an axis may be partial): cdims[a] = ceil(mask_size[a] / 4).  Cell (i, j, k) is stored at d_out[(i * cdims[1] + j) *
+ * cdims[2] + k] and holds the Chebyshev distance, in cells, to the nearest cell that contains an occupied voxel: 0 for
+ * such a cell, and 49 for every cell with no occupied cell within 48 cells (also every cell of an empty mask).
+ *   d_out: device buffer of n bytes, n >= cdims[0] * cdims[1] * cdims[2].  cdims (host) receives the cell dimensions.
+ *   A scene without the field returns K4_ERR_UNSUPPORTED with cdims zeroed: DirectContractedVoxGO, a scene created with
+ *   K4_NO_SKIP set, and one whose mask has a single voxel on some axis (xyz2ijk_scale 0 there: every point maps to that
+ *   voxel, and the skip geometry needs 1 / scale).  Arguments are checked before any CUDA call (K4_ERR_INVALID_ARG).  The copy
+ *   is a synchronous cudaMemcpy: the call returns when d_out holds the field.
+ */
+K4_API int k4_testing_skip_field(const k4_scene* scene, uint8_t* d_out, int64_t n, int32_t cdims[3]);
+
 #ifdef __cplusplus
 }
 #endif

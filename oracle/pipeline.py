@@ -233,12 +233,30 @@ def _early_out_counts(ids_m, ids_d, ids_a, i_end, alphainv_last, N):
     return out
 
 
-def _trace(trace, ray_id, weights, rgb_feat, diffuse):
-    """Record the surviving samples of a forward pass with an rgbnet: ray_id [S], weights [S], the rgbnet's inputs
-    rgb_feat [S, dim0] and, for rgbnet_direct=False, the diffuse logits [S, 3] added before the sigmoid (else None)."""
+def _trace(trace, ray_id, weights, rgb_feat, diffuse, step_id, s):
+    """Record the shaded samples of a forward pass: ray_id [S], weights [S], the rgbnet's inputs rgb_feat [S, dim0] (the
+    k0 colour logits [S, 3] for a model without an rgbnet) and, for rgbnet_direct=False, the diffuse logits [S, 3] added
+    before the sigmoid (else None); step_id [S] and the depth coordinate s [S] of each."""
     if trace is not None:
         trace.update(ray_id=ray_id.clone(), weights=weights.clone(), rgb_feat=rgb_feat.clone(),
-                     diffuse=None if diffuse is None else diffuse.clone())
+                     diffuse=None if diffuse is None else diffuse.clone(), step_id=step_id.clone(), s=s.clone())
+
+
+def _trace_occupied(trace, ray_id, step_id, pts, density, alpha):
+    """Record every occupied sample (the mask lookup hit it), in ray and step order: its ray, step, position, density as
+    it enters raw2alpha (before the shift) and alpha."""
+    if trace is not None:
+        trace['occupied'] = dict(ray_id=ray_id.clone(), step_id=step_id.clone(), pts=pts.clone(),
+                                 density=density.flatten().clone(), alpha=alpha.flatten().clone())
+
+
+def _trace_composited(trace, ray_id, step_id, alpha, T, i_end):
+    """Record the samples alpha2weight composites (the alpha threshold's survivors, or every occupied sample without a
+    threshold): ray, step, alpha and the transmittance T in front of the sample; and per ray i_end, one past the last
+    sample it composited before the T < 1e-3 early-out."""
+    if trace is not None:
+        trace['composited'] = dict(ray_id=ray_id.clone(), step_id=step_id.clone(), alpha=alpha.clone(), T=T.clone(),
+                                   i_end=i_end.clone())
 
 
 def _add_stats(stats, ids_m, ids_d, S_c, ray_stats, ray_id_c, N):
@@ -282,6 +300,7 @@ def dvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **re
 
     density = dense_grid(st['density'], ray_pts, st['xyz_min'], st['xyz_max'])
     alpha = ops.raw2alpha(density.flatten().contiguous(), float(st['act_shift']), interval)[1].reshape(density.shape)
+    _trace_occupied(trace, ray_id, step_id, ray_pts, density, alpha)
     if st['fast_color_thres'] > 0:
         mask2 = (alpha > st['fast_color_thres'])
         ray_pts = ray_pts[mask2]
@@ -289,7 +308,8 @@ def dvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **re
         step_id = step_id[mask2]
         alpha = alpha[mask2]
 
-    weights, _, alphainv_last, _, i_end = ops.alpha2weight(alpha.contiguous(), ray_id.contiguous(), N)
+    weights, T_in, alphainv_last, _, i_end = ops.alpha2weight(alpha.contiguous(), ray_id.contiguous(), N)
+    _trace_composited(trace, ray_id, step_id, alpha, T_in, i_end)
     ray_stats = _early_out_counts(ids_m, ids_d, (ray_id, step_id), i_end, alphainv_last, N) if stats is not None else None
     if st['fast_color_thres'] > 0:
         mask3 = (weights > st['fast_color_thres'])
@@ -299,9 +319,11 @@ def dvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **re
         ray_id = ray_id[mask3]
         step_id = step_id[mask3]
     S_c = ray_pts.shape[0]
+    s = (step_id + 0.5) / N_samples
 
     k0 = dense_grid(st['k0'], ray_pts, st['xyz_min'], st['xyz_max'])
     if st['rgbnet'] is None:
+        _trace(trace, ray_id, weights, k0, None, step_id, s)
         rgb_raw = torch.sigmoid(k0)
     else:
         if st['rgbnet_direct']:
@@ -313,7 +335,7 @@ def dvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **re
         viewdirs_emb = torch.cat([viewdirs, viewdirs_emb.sin(), viewdirs_emb.cos()], -1)
         viewdirs_emb = viewdirs_emb.flatten(0, -2)[ray_id]
         rgb_feat = torch.cat([k0_view, viewdirs_emb], -1)
-        _trace(trace, ray_id, weights, rgb_feat, None if st['rgbnet_direct'] else k0_diffuse)
+        _trace(trace, ray_id, weights, rgb_feat, None if st['rgbnet_direct'] else k0_diffuse, step_id, s)
         rgb_logit = mlp(st['rgbnet'], rgb_feat)
         if st['rgbnet_direct']:
             rgb_raw = torch.sigmoid(rgb_logit)
@@ -323,7 +345,6 @@ def dvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **re
     rgb_feature = _segment_sum(weights.unsqueeze(-1) * rgb_raw, ray_id, torch.zeros([N, 3], device=dev))
     rgb_marched = rgb_feature                      # alias, lib/dvgo.py:425
     rgb_marched += (alphainv_last.unsqueeze(-1) * render_kwargs['bg'])
-    s = (step_id + 0.5) / N_samples
     ret = {
         'alphainv_last': alphainv_last, 'weights': weights, 'rgb_marched': rgb_marched,
         'rgb_feature': rgb_feature, 'raw_alpha': alpha, 'raw_rgb': rgb_raw, 'ray_id': ray_id,
@@ -367,6 +388,7 @@ def dmpigo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **
     density = dense_grid(st['density'], ray_pts, st['xyz_min'], st['xyz_max']) + \
         dense_grid(st['act_shift_grid'], ray_pts, st['xyz_min'], st['xyz_max'])
     alpha = ops.raw2alpha(density.flatten().contiguous(), 0, interval)[1].reshape(density.shape)
+    _trace_occupied(trace, ray_id, step_id, ray_pts, density, alpha)
     if st['fast_color_thres'] > 0:
         mask2 = (alpha > st['fast_color_thres'])
         ray_pts = ray_pts[mask2]
@@ -374,7 +396,8 @@ def dmpigo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **
         step_id = step_id[mask2]
         alpha = alpha[mask2]
 
-    weights, _, alphainv_last, _, i_end = ops.alpha2weight(alpha.contiguous(), ray_id.contiguous(), N)
+    weights, T_in, alphainv_last, _, i_end = ops.alpha2weight(alpha.contiguous(), ray_id.contiguous(), N)
+    _trace_composited(trace, ray_id, step_id, alpha, T_in, i_end)
     ray_stats = _early_out_counts(ids_m, ids_d, (ray_id, step_id), i_end, alphainv_last, N) if stats is not None else None
     if st['fast_color_thres'] > 0:
         mask3 = (weights > st['fast_color_thres'])
@@ -384,10 +407,12 @@ def dmpigo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **
         alpha = alpha[mask3]
         weights = weights[mask3]
     S_c = ray_pts.shape[0]
+    s = (step_id + 0.5) / N_samples
 
     vox_emb = dense_grid(st['k0'], ray_pts, st['xyz_min'], st['xyz_max'])
     pe_spa = ((ray_pts - st['xyz_min']) / (st['xyz_max'] - st['xyz_min'])).flip((-1,)) * 2 - 1
     if st['rgbnet'] is None:
+        _trace(trace, ray_id, weights, vox_emb, None, step_id, s)
         rgb_raw = torch.sigmoid(vox_emb)
     else:
         viewdirs_emb = (viewdirs.unsqueeze(-1) * st['viewfreq']).flatten(-2)
@@ -396,14 +421,13 @@ def dmpigo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **
         pe_emb = (pe_spa.unsqueeze(-1) * st['posfreq']).flatten(-2)
         pe_emb = torch.cat([pe_spa, pe_emb.sin(), pe_emb.cos()], -1)
         rgb_feat = torch.cat([vox_emb, pe_emb, viewdirs_emb], -1)
-        _trace(trace, ray_id, weights, rgb_feat, None)
+        _trace(trace, ray_id, weights, rgb_feat, None, step_id, s)
         rgb_logit = mlp(st['rgbnet'], rgb_feat)
         rgb_raw = torch.sigmoid(rgb_logit)
 
     rgb_feature = _segment_sum(weights.unsqueeze(-1) * rgb_raw, ray_id, torch.zeros([N, 3], device=dev))
     rgb_marched = rgb_feature                      # alias, lib/dmpigo.py:392
     rgb_marched += (alphainv_last.unsqueeze(-1) * render_kwargs['bg'])   # global_step is None branch, :397
-    s = (step_id + 0.5) / N_samples
     ret = {
         'alphainv_last': alphainv_last, 'weights': weights, 'rgb_marched': rgb_marched,
         'rgb_feature': rgb_feature, 'raw_alpha': alpha, 'raw_rgb': rgb_raw, 'ray_id': ray_id,
@@ -458,29 +482,32 @@ def dcvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **r
 
     density = dense_grid(st['density'], ray_pts, st['xyz_min'], st['xyz_max'])
     alpha = ops.raw2alpha(density.flatten().contiguous(), float(st['act_shift']), interval)[1].reshape(density.shape)
+    _trace_occupied(trace, ray_id, step_id, ray_pts, density, alpha)
     if st['fast_color_thres'] > 0:
         m2 = (alpha > st['fast_color_thres'])
         ray_pts, tt, ray_id, step_id, alpha = ray_pts[m2], tt[m2], ray_id[m2], step_id[m2], alpha[m2]
-    weights, _, alphainv_last, _, i_end = ops.alpha2weight(alpha.contiguous(), ray_id.contiguous(), N)
+    weights, T_in, alphainv_last, _, i_end = ops.alpha2weight(alpha.contiguous(), ray_id.contiguous(), N)
+    _trace_composited(trace, ray_id, step_id, alpha, T_in, i_end)
     ray_stats = _early_out_counts(ids_m, ids_d, (ray_id, step_id), i_end, alphainv_last, N) if stats is not None else None
     if st['fast_color_thres'] > 0:
         m3 = (weights > st['fast_color_thres'])
         ray_pts, tt, ray_id, step_id, alpha, weights = ray_pts[m3], tt[m3], ray_id[m3], step_id[m3], alpha[m3], weights[m3]
     S_c = ray_pts.shape[0]
+    s = 1 - 1 / (1 + tt)
 
     k0 = dense_grid(st['k0'], ray_pts, st['xyz_min'], st['xyz_max'])
     if st['rgbnet'] is None:
+        _trace(trace, ray_id, weights, k0, None, step_id, s)
         rgb = torch.sigmoid(k0)
     else:
         viewdirs_emb = (viewdirs.unsqueeze(-1) * st['viewfreq']).flatten(-2)
         viewdirs_emb = torch.cat([viewdirs, viewdirs_emb.sin(), viewdirs_emb.cos()], -1)
         viewdirs_emb = viewdirs_emb.flatten(0, -2)[ray_id]
         rgb_feat = torch.cat([k0, viewdirs_emb], -1)
-        _trace(trace, ray_id, weights, rgb_feat, None)
+        _trace(trace, ray_id, weights, rgb_feat, None, step_id, s)
         rgb = torch.sigmoid(mlp(st['rgbnet'], rgb_feat))
     rgb_marched = _segment_sum(weights.unsqueeze(-1) * rgb, ray_id, torch.zeros([N, 3], device=dev))
     rgb_marched += (alphainv_last.unsqueeze(-1) * render_kwargs['bg'])
-    s = 1 - 1 / (1 + tt)
     ret = {'alphainv_last': alphainv_last, 'weights': weights, 'rgb_marched': rgb_marched, 'rgb_feature': rgb_marched,
            'raw_alpha': alpha, 'raw_rgb': rgb, 'ray_id': ray_id, 'step_id': step_id, 'n_max': n_max, 't': tt, 's': s}
     if render_kwargs.get('render_depth', False):
@@ -492,7 +519,8 @@ def dcvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **r
 
 
 def forward(st, rays_o, rays_d, viewdirs, ops, stats=None, trace=None, **render_kwargs):
-    """trace: optional dict that receives the samples shaded by the rgbnet (see _trace)."""
+    """trace: optional dict that receives the shaded samples (see _trace), and under 'occupied' / 'composited' the
+    samples that hit the occupancy mask and those alpha2weight composited (_trace_occupied / _trace_composited)."""
     if st['kind'] == 'dcvgo':
         return dcvgo_forward(st, rays_o, rays_d, viewdirs, ops, stats=stats, trace=trace, **render_kwargs)
     fn = dvgo_forward if st['kind'] == 'dvgo' else dmpigo_forward

@@ -198,3 +198,24 @@ def test_testing_rgbnet_validates_arguments_without_a_gpu():
     for mode in range(5):
         assert lib.k4_testing_rgbnet(C.addressof(scene), C.byref(args(mode=mode)), C.byref(g), None) == -2, mode
         assert g.value == 0
+
+
+def test_testing_skip_field_validates_arguments_without_a_gpu():
+    """k4_testing_skip_field (the empty-space-skipping field for the GPU tests): bad arguments are reported as
+    K4_ERR_INVALID_ARG before any CUDA call, and cdims is zeroed.  The scene here is a zero-filled host block: a scene
+    without a field, which is K4_ERR_UNSUPPORTED once the arguments are valid."""
+    from k4nerf import _lib
+    C = ctypes
+    lib = _lib.lib
+    buf = C.create_string_buffer(64)
+    scene = C.create_string_buffer(1 << 16)
+    cd = (C.c_int32 * 3)(7, 7, 7)
+    for sc, out, n, dims in ((None, buf, 64, cd), (scene, None, 64, cd), (scene, buf, 0, cd), (scene, buf, -5, cd),
+                             (scene, buf, 64, None)):
+        cd[:] = [7, 7, 7]
+        assert lib.k4_testing_skip_field(sc and C.addressof(sc), out and C.addressof(out), n, dims) == -1, (sc, out, n, dims)
+        if dims is not None:
+            assert list(cd) == [0, 0, 0]
+    cd[:] = [7, 7, 7]
+    assert lib.k4_testing_skip_field(C.addressof(scene), C.addressof(buf), 64, cd) == -2
+    assert list(cd) == [0, 0, 0]
