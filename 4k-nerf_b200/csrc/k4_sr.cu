@@ -1438,10 +1438,11 @@ extern "C" int k4_srnet_destroy(k4_srnet* n) {
 extern "C" int k4_srnet_create(const k4_srnet_desc* d, k4_stream_t stream, k4_srnet** out) {
     if (!d || !out || !d->h_params) return K4_ERR_INVALID_ARG;
     *out = nullptr;
-    if (d->num_feat != 64 || d->num_grow_ch != 32 || d->num_cond != 1 || d->n_in_colors != 3 || d->scale != 4 ||
+    if (d->num_feat != 64 || d->num_grow_ch != 32 || d->num_cond != 1 || d->n_in_colors != 3 || (d->scale != 4 && d->scale != 1) ||
         d->num_block < 1 || d->num_block > 32)
-        return K4_ERR_UNSUPPORTED;          // the shipped configuration (run_sr.py:1353); others are not built
-    const int expect = 2 * (1 + 4 + d->num_block * (3 * 13 + 4) + 4 + 5);
+        return K4_ERR_UNSUPPORTED;          // the shipped configurations (run_sr.py:1353; x1 as in the 1x configs); others are not built
+    const bool up = d->scale == 4;          // x1 registers no conv_up1 / conv_up2 (lib/sr_esrnet.py:430-433)
+    const int expect = 2 * (1 + 4 + d->num_block * (3 * 13 + 4) + 4 + (up ? 5 : 3));
     if (d->n_params != expect) return K4_ERR_INVALID_ARG;
     for (int i = 0; i < d->n_params; ++i) if (!d->h_params[i]) return K4_ERR_INVALID_ARG;
     int st = k4_device_check();
@@ -1450,7 +1451,7 @@ extern "C" int k4_srnet_create(const k4_srnet_desc* d, k4_stream_t stream, k4_sr
     k4_srnet* n = new (std::nothrow) k4_srnet();
     if (!n) return K4_ERR_INVALID_ARG;
     memset(n, 0, sizeof(*n));
-    n->num_feat = 64; n->num_block = d->num_block; n->num_grow = 32; n->num_cond = 1; n->n_in = 3; n->scale = 4;
+    n->num_feat = 64; n->num_block = d->num_block; n->num_grow = 32; n->num_cond = 1; n->n_in = 3; n->scale = d->scale;
     const float* const* P = d->h_params;
     int k = 0;
 #define SR_TRY(x) do { st = (x); if (st != K4_OK) { k4_srnet_destroy(n); return st; } } while (0)
@@ -1469,8 +1470,10 @@ extern "C" int k4_srnet_create(const k4_srnet_desc* d, k4_stream_t stream, k4_sr
     }
     SR_TRY(make_sft(n, n->sftbody, P + k, 64, s)); k += 8;
     SR_TRY(make_conv(n, n->conv_body, P[k], P[k + 1], 64, 64, s)); SR_TRY(make_conv_k64(n, n->conv_body, P[k], 64, 64, false, s)); k += 2;
-    SR_TRY(make_conv(n, n->conv_up1, P[k], P[k + 1], 64, 64, s)); SR_TRY(make_conv_phases(n, n->conv_up1, P[k], 64, 64, s)); SR_TRY(make_conv_k64(n, n->conv_up1, P[k], 64, 64, true, s)); k += 2;
-    SR_TRY(make_conv(n, n->conv_up2, P[k], P[k + 1], 64, 64, s)); SR_TRY(make_conv_phases(n, n->conv_up2, P[k], 64, 64, s)); SR_TRY(make_conv_k64(n, n->conv_up2, P[k], 64, 64, true, s)); k += 2;
+    if (up) {
+        SR_TRY(make_conv(n, n->conv_up1, P[k], P[k + 1], 64, 64, s)); SR_TRY(make_conv_phases(n, n->conv_up1, P[k], 64, 64, s)); SR_TRY(make_conv_k64(n, n->conv_up1, P[k], 64, 64, true, s)); k += 2;
+        SR_TRY(make_conv(n, n->conv_up2, P[k], P[k + 1], 64, 64, s)); SR_TRY(make_conv_phases(n, n->conv_up2, P[k], 64, 64, s)); SR_TRY(make_conv_k64(n, n->conv_up2, P[k], 64, 64, true, s)); k += 2;
+    }
     SR_TRY(make_conv(n, n->conv_hr, P[k], P[k + 1], 64, 64, s)); SR_TRY(make_conv_k64(n, n->conv_hr, P[k], 64, 64, false, s)); k += 2;
     SR_TRY(make_conv(n, n->conv_last, P[k], P[k + 1], 3, 64, s)); SR_TRY(make_conv_k64(n, n->conv_last, P[k], 3, 64, false, s)); k += 2;
 #undef SR_TRY
@@ -1478,9 +1481,9 @@ extern "C" int k4_srnet_create(const k4_srnet_desc* d, k4_stream_t stream, k4_sr
     return K4_OK;
 }
 
-// workspace layout for an h x w tile (P = h*w LR pixels)
+// workspace layout for an h x w tile (P = h*w LR pixels) of a x`scale` net: x1 has no up1 / up2, and hr is at LR
 struct SrWs { size_t in16, cond32, cond16, feat, trunkA, trunkB, cat, cat2, sbody, bf, up1, up2, hr, total; };
-static SrWs sr_ws(int h, int w) {
+static SrWs sr_ws(int h, int w, int scale) {
     const size_t P = (size_t)h * w;
     SrWs o; size_t off = 0;
     auto take = [&](size_t b) { size_t r = off; off += (b + 255) & ~(size_t)255; return r; };
@@ -1488,14 +1491,16 @@ static SrWs sr_ws(int h, int w) {
     o.trunkA = take(P * 64 * 4); o.trunkB = take(P * 64 * 4); o.cat = take(P * 192 * 2);
     o.cat2 = take(P * 192 * 2); o.cond16 = take(P * 32 * 2);         // fused SFT epilogues: dense blocks alternate between two concat buffers
     o.sbody = take(P * 64 * 2); o.bf = take(P * 64 * 2);
-    o.up1 = take(P * 4 * 64 * 2); o.up2 = take(P * 16 * 64 * 2); o.hr = take(P * 16 * 64 * 2);
+    o.up1 = o.up2 = 0;
+    if (scale == 4) { o.up1 = take(P * 4 * 64 * 2); o.up2 = take(P * 16 * 64 * 2); }
+    o.hr = take(P * scale * scale * 64 * 2);
     o.total = off;
     return o;
 }
 
-extern "C" size_t k4_srnet_workspace_bytes(const k4_srnet*, int32_t h, int32_t w) {
+extern "C" size_t k4_srnet_workspace_bytes(const k4_srnet* n, int32_t h, int32_t w) {
     if (h <= 0 || w <= 0) return 0;
-    return sr_ws(h, w).total;
+    return sr_ws(h, w, n ? n->scale : 4).total;          // no net: the x4 layout, the largest of the built scales
 }
 
 // Rows [lo, hi) of an h-row tile that a layer must produce when `r` more rows of receptive field follow it
@@ -1514,7 +1519,8 @@ static int srnet_forward_roi_impl(const k4_srnet* n, const float* d_x, const flo
     if (n_extra < 0 || n_extra > K4_MAX_PEERS - 1 || (n_extra > 0 && !h_extra)) return K4_ERR_INVALID_ARG;
     for (int e = 0; e < n_extra; ++e) if (!h_extra[e]) return K4_ERR_INVALID_ARG;
     if (keep_y0 < 0 || keep_y1 > h || keep_y0 >= keep_y1 || keep_x0 < 0 || keep_x1 > w || keep_x0 >= keep_x1) return K4_ERR_INVALID_ARG;
-    const SrWs L = sr_ws(h, w);
+    const int sc = n->scale;
+    const SrWs L = sr_ws(h, w, sc);
     if (!d_ws || ws_bytes < L.total) return K4_ERR_WORKSPACE;
     cudaStream_t s = (cudaStream_t)stream;
     unsigned char* ws = (unsigned char*)d_ws;
@@ -1528,10 +1534,12 @@ static int srnet_forward_roi_impl(const k4_srnet* n, const float* d_x, const flo
     const char* fenv = getenv("K4_SR_FUSE_SFT");                   // read per call: tests compare both structures in one process
     const bool fuse = !(fenv && fenv[0] == '0') && !sr_no_tma();
     const int ky0 = keep_y0, ky1 = keep_y1;
-    // Remaining receptive radius (LR rows) behind each layer, from the output backwards: conv_last / conv_hr / up2 / up1
-    // need 1/4 + 1/4 + 1/4 + 1/2 LR rows (handled exactly in high-resolution rows below), conv_body 1, every 3x3 conv of a
-    // residual dense block 1 (SFT layers 0), conv_first 1: the trunk entering conv_body's SFT is needed on rows(3), the
-    // output of the k-th dense block from the end on rows(3 + 5k), conv_first's on rows(3 + 5 * 3 * num_block).
+    // Remaining receptive radius (LR rows) behind each layer, from the output backwards: at x4 conv_last / conv_hr / up2 / up1
+    // need 1/4 + 1/4 + 1/4 + 1/2 LR rows (handled exactly in high-resolution rows below), at x1 conv_last / conv_hr run at LR
+    // and need 1 + 1; either way conv_body's output bf is needed on rows(2), so what follows is the same for both scales:
+    // conv_body 1, every 3x3 conv of a residual dense block 1 (SFT layers 0), conv_first 1: the trunk entering conv_body's SFT
+    // is needed on rows(3), the output of the k-th dense block from the end on rows(3 + 5k), conv_first's on
+    // rows(3 + 5 * 3 * num_block).
     const int nrdb = 3 * n->num_block;
     int st;
 #define SR_DO(x) do { st = (x); if (st != K4_OK) return st; } while (0)
@@ -1647,24 +1655,27 @@ static int srnet_forward_roi_impl(const k4_srnet* n, const float* d_x, const flo
             SR_DO(run_conv(n->conv_body, p, s));
         }
     }
-    {   // upsample x2 (nearest) + conv + lrelu, twice; conv_hr + lrelu; conv_last (rows in the layer's own resolution)
-        ConvParams p = c0; p.H = 2 * h; p.W = 2 * w; p.upsample = 1; p.src = bf; p.src_cstride = 64; p.mode = SRM_STORE_F16; p.lrelu = 0.2f;
-        p.dst_h = up1; p.dst_cstride = 64;
+    {   // x4: upsample x2 (nearest) + conv + lrelu, twice; then conv_hr + lrelu and conv_last at the output resolution
+        // (x4: 4h x 4w from up2; x1: h x w straight from bf), rows in the layer's own resolution
+        ConvParams p = c0; p.src = bf; p.src_cstride = 64; p.mode = SRM_STORE_F16; p.lrelu = 0.2f; p.dst_cstride = 64;
         auto clip = [](int v, int hi) { return v < 0 ? 0 : (v > hi ? hi : v); };
-        p.H = h; p.W = w;                                       // iterate over the SOURCE grid, write the 2x grid
-        p.y_lo = clip(ky0 - 1, h); p.y_hi = clip(ky1 + 1, h);                        // -> up1 rows [2ky0-2, 2ky1+2)
-        SR_DO(run_conv_up2x(n->conv_up1, p, s));
-        p.H = 2 * h; p.W = 2 * w; p.src = up1; p.dst_h = up2;
-        p.y_lo = clip(2 * ky0 - 1, 2 * h); p.y_hi = clip(2 * ky1 + 1, 2 * h);        // -> up2 rows [4ky0-2, 4ky1+2)
-        SR_DO(run_conv_up2x(n->conv_up2, p, s));
-        p.H = 4 * h; p.W = 4 * w;
-        p.upsample = 0; p.src = up2; p.dst_h = hr;
-        p.y_lo = clip(4 * ky0 - 1, 4 * h); p.y_hi = clip(4 * ky1 + 1, 4 * h);
+        if (sc == 4) {
+            p.upsample = 1; p.dst_h = up1;
+            p.H = h; p.W = w;                                   // iterate over the SOURCE grid, write the 2x grid
+            p.y_lo = clip(ky0 - 1, h); p.y_hi = clip(ky1 + 1, h);                    // -> up1 rows [2ky0-2, 2ky1+2)
+            SR_DO(run_conv_up2x(n->conv_up1, p, s));
+            p.H = 2 * h; p.W = 2 * w; p.src = up1; p.dst_h = up2;
+            p.y_lo = clip(2 * ky0 - 1, 2 * h); p.y_hi = clip(2 * ky1 + 1, 2 * h);    // -> up2 rows [4ky0-2, 4ky1+2)
+            SR_DO(run_conv_up2x(n->conv_up2, p, s));
+            p.upsample = 0; p.src = up2;
+        }
+        p.H = sc * h; p.W = sc * w; p.dst_h = hr;
+        p.y_lo = clip(sc * ky0 - 1, sc * h); p.y_hi = clip(sc * ky1 + 1, sc * h);
         SR_DO(run_conv(n->conv_hr, p, s));
-        ConvParams q = c0; q.H = 4 * h; q.W = 4 * w; q.src = hr; q.src_cstride = 64; q.mode = SRM_OUT_NCHW; q.out_nchw = d_out; q.n_valid = 3;
-        q.y_lo = 4 * ky0; q.y_hi = 4 * ky1;
+        ConvParams q = c0; q.H = sc * h; q.W = sc * w; q.src = hr; q.src_cstride = 64; q.mode = SRM_OUT_NCHW; q.out_nchw = d_out; q.n_valid = 3;
+        q.y_lo = sc * ky0; q.y_hi = sc * ky1;
         q.out_ps = out_plane_stride; q.out_rs = out_row_stride;
-        q.crop_y0 = 4 * ky0; q.crop_y1 = 4 * ky1; q.crop_x0 = 4 * keep_x0; q.crop_x1 = 4 * keep_x1;
+        q.crop_y0 = sc * ky0; q.crop_y1 = sc * ky1; q.crop_x0 = sc * keep_x0; q.crop_x1 = sc * keep_x1;
         q.n_out_extra = n_extra;
         for (int e = 0; e < n_extra; ++e) q.out_extra[e] = h_extra[e];
         SR_DO(run_conv(n->conv_last, q, s));
@@ -1692,7 +1703,9 @@ extern "C" int k4_srnet_forward_roi_peers(const k4_srnet* n, const float* d_x, c
 
 extern "C" int k4_srnet_forward(const k4_srnet* n, const float* d_x, const float* d_cond, int32_t h, int32_t w,
                                 float* d_out, void* d_ws, size_t ws_bytes, k4_stream_t stream) {
-    return k4_srnet_forward_roi(n, d_x, d_cond, h, w, 0, h, 0, w, d_out, (int64_t)16 * h * w, (int64_t)4 * w, d_ws, ws_bytes, stream);
+    if (!n) return K4_ERR_INVALID_ARG;
+    const int64_t sc = n->scale;
+    return k4_srnet_forward_roi(n, d_x, d_cond, h, w, 0, h, 0, w, d_out, sc * sc * h * w, sc * w, d_ws, ws_bytes, stream);
 }
 
 // One decoder layer for the test suite: a throw-away k4_srnet holds the packs (make_conv & co., as k4_srnet_create

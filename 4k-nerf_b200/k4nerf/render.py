@@ -160,10 +160,11 @@ def render_frame_4k(model, net_sr, H, W, K, c2w, ndc, render_kwargs, test_tile=5
                     flip_x=False, flip_y=False):
     """One full 4K-NeRF frame, device resident (SURVEY.md section 8 f-1): rays generated on the
     device, one fused marcher launch at HxW, ``rgb_feature`` + ``depth`` handed to the VC-Decoder
-    without the numpy round trip of run_sr.py:130-133,1362-1367, x4 decode with the reference's tile
-    geometry (``--test_tile``), optional ``to8b`` quantisation (lib/utils.py:20) on the device.
+    without the numpy round trip of run_sr.py:130-133,1362-1367, x``s`` decode (``s = net_sr.scale``: 4, or 1 for the
+    1x configs) with the reference's tile geometry (``--test_tile``), optional ``to8b`` quantisation (lib/utils.py:20)
+    on the device.
 
-    Returns ``(sr [3,4H,4W] float32 in [0,1] or uint8 [4H,4W,3], lr dict)`` -- same values as
+    Returns ``(sr [3,s*H,s*W] float32 in [0,1] or uint8 [s*H,s*W,3], lr dict)`` -- same values as
     ``render_viewpoints_sr`` followed by ``SFTNet.tile_process`` and ``clamp(0,1)``."""
     rays_o, rays_d, viewdirs = dvgo.get_rays_of_a_view(
         H, W, K, torch.as_tensor(np.asarray(c2w), dtype=torch.float32), ndc,
@@ -186,8 +187,8 @@ def render_frame_4k_sharded(model, net_sr, H, W, K, c2w, ndc, render_kwargs, tes
     """:func:`render_frame_4k` across the ranks of ``group`` (one process per GPU, scene and decoder
     replicated; SURVEY.md section 8e / config 5): every rank marches its 8-row blocks of the LR frame
     (one all-gather of the packed ``[rgb|depth|alphainv]`` rows), then decodes its share of the
-    reference tiles / tile row-parts (one all-gather of the x4 blocks).  Every rank returns the full
-    frame; values are identical to the single-GPU :func:`render_frame_4k`.  The LR dict's tensors are views of the
+    reference tiles / tile row-parts (one all-gather of the decoded blocks, x``net_sr.scale``).  Every rank returns the
+    full frame; values are identical to the single-GPU :func:`render_frame_4k`.  The LR dict's tensors are views of the
     cached :class:`k4nerf.dist.CyclicFrame` buffer (no allocation per frame): valid until the next call with the same
     (H, W, group)."""
     from . import dist as kdist

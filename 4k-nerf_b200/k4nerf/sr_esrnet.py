@@ -6,6 +6,7 @@ no torch op runs in ``forward``."""
 import ctypes as C
 import math
 from copy import deepcopy
+from fractions import Fraction
 
 import torch
 from torch import nn
@@ -67,15 +68,17 @@ class _NetHandle:
 class SFTNet(nn.Module):
     def __init__(self, n_in_colors, scale, num_feat=64, num_block=5, num_grow_ch=32, num_cond=1, dswise=False):
         super().__init__()
-        if dswise or n_in_colors != 3 or scale != 4 or num_feat != 64 or num_grow_ch != 32 or num_cond != 1:
-            raise NotImplementedError('k4nerf builds the shipped VC-Decoder: SFTNet(3, 4, 64, n, 32, 1) (run_sr.py:1353)')
+        if dswise or n_in_colors != 3 or scale not in (1, 4) or num_feat != 64 or num_grow_ch != 32 or num_cond != 1:
+            raise NotImplementedError('k4nerf builds the shipped VC-Decoders: SFTNet(3, 4, 64, n, 32, 1) (run_sr.py:1353) and '
+                                      'SFTNet(3, 1, 64, n, 32, 1) (the 1x configs)')
         self.scale = scale
         self.dswise = dswise
         self.conv_first = nn.Conv2d(n_in_colors, num_feat, 3, 1, 1)
         self.body = nn.Sequential(*[RRDB_SFT(num_feat=num_feat, num_grow_ch=num_grow_ch) for _ in range(num_block)])
         self.conv_body = nn.Conv2d(num_feat, num_feat, 3, 1, 1)
-        self.conv_up1 = nn.Conv2d(num_feat, num_feat, 3, 1, 1)
-        self.conv_up2 = nn.Conv2d(num_feat, num_feat, 3, 1, 1)
+        if scale == 4:                     # x1 registers no upsampling convs (lib/sr_esrnet.py:430-433)
+            self.conv_up1 = nn.Conv2d(num_feat, num_feat, 3, 1, 1)
+            self.conv_up2 = nn.Conv2d(num_feat, num_feat, 3, 1, 1)
         self.conv_hr = nn.Conv2d(num_feat, num_feat, 3, 1, 1)
         self.conv_last = nn.Conv2d(num_feat, 3, 3, 1, 1)
         self.sftbody = SFTLayer(num_feat, num_grow_ch)
@@ -93,7 +96,10 @@ class SFTNet(nn.Module):
             for rdb in (blk.rdb1, blk.rdb2, blk.rdb3):
                 cs += [rdb.conv1, rdb.conv2, rdb.conv3, rdb.conv4, rdb.conv5] + rdb.sft0.convs() + rdb.sft1.convs()
             cs += blk.sft0.convs()
-        cs += self.sftbody.convs() + [self.conv_body, self.conv_up1, self.conv_up2, self.conv_hr, self.conv_last]
+        cs += self.sftbody.convs() + [self.conv_body]
+        if self.scale == 4:
+            cs += [self.conv_up1, self.conv_up2]
+        cs += [self.conv_hr, self.conv_last]
         return cs
 
     def _get_net(self):
@@ -129,9 +135,10 @@ class SFTNet(nn.Module):
 
     @torch.no_grad()
     def forward_roi(self, x, cond, keep, out, ws_slot=0, extra=None):
-        """The x4 pixels of LR block ``keep = (y0, y1, x0, x1)`` of tile ``x [1,3,h,w]`` / ``cond [1,1,h,w]`` written
-        into ``out``: a ``[3, 4(y1-y0), 4(x1-x0)]`` fp32 CUDA view with unit stride along x (typically a window of the
-        frame).  Same values as ``forward(x, cond)[0, :, 4y0:4y1, 4x0:4x1]``; every layer computes only the rows inside the
+        """The output pixels (``s = self.scale`` per LR pixel and axis) of LR block ``keep = (y0, y1, x0, x1)`` of tile
+        ``x [1,3,h,w]`` / ``cond [1,1,h,w]`` written into ``out``: a ``[3, s(y1-y0), s(x1-x0)]`` fp32 CUDA view with unit
+        stride along x (typically a window of the frame).  Same values as ``forward(x, cond)[0, :, s*y0:s*y1, s*x0:s*x1]``;
+        every layer computes only the rows inside the
         remaining receptive field of the kept rows (k4_srnet_forward_roi).  Runs on the current stream.  ``extra``: device
         pointers (ints) of the same window in other ranks' peer-mapped frames -- the last convolution stores the block there
         too (k4_srnet_forward_roi_peers)."""
@@ -200,7 +207,7 @@ class SFTNet(nn.Module):
 
     @torch.no_grad()
     def forward(self, x, cond, fea=None):
-        """x [1,3,h,w], cond [1,1,h,w] (CUDA, fp32) -> [1,3,4h,4w]  (lib/sr_esrnet.py:446-465)."""
+        """x [1,3,h,w], cond [1,1,h,w] (CUDA, fp32) -> [1,3,s*h,s*w], s = self.scale  (lib/sr_esrnet.py:446-465)."""
         if fea is not None:
             raise NotImplementedError('the `fea` branch needs conv_prefea (n_in_colors > 3), not in the shipped config')
         require_cuda(x, cond)
@@ -241,10 +248,13 @@ class SFTNet(nn.Module):
 
     def receptive_halo(self):
         """LR rows a decoded pixel can depend on above/below it: conv_first/CondNet.0 (1) + 15 3x3 convs
-        per RRDB_SFT + conv_body (1) + the four 3x3 convs after the nearest upsamplings (1/2 + 3/4 LR
-        pixels), rounded up to an even count.  Row parts of a tile cut with this halo reproduce the
-        un-split tile exactly (dist.sr_units)."""
-        r = 1 + 15 * len(self.body) + 1 + 2
+        per RRDB_SFT + conv_body (1) + the tail, rounded up to an even count.  The tail is the 3x3 convs behind
+        conv_body, each 1 row at its own resolution: at x4 conv_up1 (1/2 LR row) and conv_up2, conv_hr, conv_last
+        (1/4 each), 5/4 -> 2 LR rows; at x1 conv_hr + conv_last at LR, 2 rows.  So the halo is 80 for 5 blocks at
+        either scale.  Row parts of a tile cut with this halo reproduce the un-split tile exactly (dist.sr_units)."""
+        res = ([2, 4] if self.scale == 4 else []) + [self.scale, self.scale]     # resolution factor of each tail conv
+        tail = math.ceil(sum(Fraction(1, f) for f in res))
+        r = 1 + 15 * len(self.body) + 1 + tail
         return r + (r & 1)
 
     def tile_process_sharded(self, img, cond, tile_size, tile_pad=10, group=None):

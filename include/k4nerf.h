@@ -214,19 +214,24 @@ K4_API int k4_make_rays_rows(const float* h_K, const float* h_c2w, int32_t H, in
                  float* d_rays_o, float* d_rays_d, float* d_viewdirs, k4_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
- * VC-Decoder: SFTNet (lib/sr_esrnet.py:400-465), the x4 SFT-RRDB upsampler that turns the marcher's
- * rgb_feature + depth images into the 4K frame (run_sr.py:1353-1387).
+ * VC-Decoder: SFTNet (lib/sr_esrnet.py:400-465), the SFT-RRDB decoder that turns the marcher's
+ * rgb_feature + depth images into the output frame (run_sr.py:1353-1387): x4, the 4K upsampler, or x1, the
+ * refinement network of the 1x configurations (no upsampling; conv_hr and conv_last run at the input resolution).
  *
  * h_params: HOST array of DEVICE pointers to the fp32 parameters (weight, bias alternating) of the
- * 229 convolutions in this fixed order -- the reference module's registration order:
+ * convolutions in this fixed order -- the reference module's registration order:
  *   conv_first; CondNet.0, CondNet.2, CondNet.4, CondNet.6;
  *   for i in blocks: for j in rdb1..rdb3: conv1..conv5,
  *                                          sft0.{SFT_scale_conv0, SFT_scale_conv1, SFT_shift_conv0, SFT_shift_conv1},
  *                                          sft1.{same four};
  *                    body.i.sft0.{same four};
- *   sftbody.{same four}; conv_body; conv_up1; conv_up2; conv_hr; conv_last.
- * Only the shipped configuration SFTNet(n_in_colors=3, scale=4, num_feat=64, num_block<=32,
- * num_grow_ch=32, num_cond=1, dswise=False) (run_sr.py:1353) is built; others return K4_ERR_UNSUPPORTED.
+ *   sftbody.{same four}; then
+ *     scale 4: conv_body; conv_up1; conv_up2; conv_hr; conv_last.
+ *     scale 1: conv_body; conv_hr; conv_last.
+ * n_params = 2 * (1 + 4 + 43 * num_block + 4 + (scale == 4 ? 5 : 3)): 229 convolutions for 5 blocks at x4, 227 at x1;
+ * a count that does not match the scale returns K4_ERR_INVALID_ARG.
+ * Only SFTNet(n_in_colors=3, scale=4 or 1, num_feat=64, num_block<=32, num_grow_ch=32, num_cond=1, dswise=False)
+ * (run_sr.py:1353) is built; other configurations, scale 2 included, return K4_ERR_UNSUPPORTED.
  */
 typedef struct k4_srnet_desc {
     int32_t n_in_colors, scale, num_feat, num_block, num_grow_ch, num_cond;
@@ -237,10 +242,13 @@ typedef struct k4_srnet_desc {
 
 K4_API int k4_srnet_create(const k4_srnet_desc* desc, k4_stream_t stream, k4_srnet** out_net);
 K4_API int k4_srnet_destroy(k4_srnet* net);
+/* Device workspace of one h x w tile for `net`'s scale (x1 needs less than x4); net == NULL gives the x4 size, which
+ * covers every built scale. */
 K4_API size_t k4_srnet_workspace_bytes(const k4_srnet* net, int32_t h, int32_t w);
 
 /* Replaces: SFTNet.forward(x, cond) (lib/sr_esrnet.py:446-465) for one tile.
- * d_x [3,h,w], d_cond [1,h,w] planar fp32 (the reference's NCHW, batch 1); d_out [3,4h,4w] fp32.
+ * d_x [3,h,w], d_cond [1,h,w] planar fp32 (the reference's NCHW, batch 1); d_out [3,s*h,s*w] fp32 with s the net's
+ * scale (4 or 1).
  * Tiling (SFTNet.tile_process, lib/sr_esrnet.py:467-527) is host logic above this call. */
 K4_API int k4_srnet_forward(const k4_srnet* net, const float* d_x, const float* d_cond, int32_t h, int32_t w,
                             float* d_out, void* d_workspace, size_t workspace_bytes, k4_stream_t stream);
@@ -248,8 +256,9 @@ K4_API int k4_srnet_forward(const k4_srnet* net, const float* d_x, const float* 
 /* The same forward when only a block of the tile's output is wanted -- what SFTNet.tile_process does with every tile
  * (lib/sr_esrnet.py:509-523 crops the 10-pixel pad away and copies the rest into the frame) and what the multi-GPU
  * decoder does with a tile's row parts.  keep_* select LR rows [keep_y0,keep_y1) x columns [keep_x0,keep_x1) of the
- * h x w input; their x4 pixels are written straight to d_out[c*out_plane_stride + Y*out_row_stride + X] with (Y, X)
- * relative to the block's first pixel (pass a pointer into the frame and the frame's strides).  Every layer computes only
+ * h x w input; their x scale pixels (x4: 4x4 per LR pixel; x1: the block 1:1) are written straight to
+ * d_out[c*out_plane_stride + Y*out_row_stride + X] with (Y, X) relative to the block's first pixel (pass a pointer into
+ * the frame and the frame's strides).  Every layer computes only
  * the rows inside the remaining receptive field of the kept rows; the values are bit-identical to k4_srnet_forward's. */
 K4_API int k4_srnet_forward_roi(const k4_srnet* net, const float* d_x, const float* d_cond, int32_t h, int32_t w,
                                 int32_t keep_y0, int32_t keep_y1, int32_t keep_x0, int32_t keep_x1,
