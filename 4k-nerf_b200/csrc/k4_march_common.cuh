@@ -127,6 +127,50 @@ __device__ __forceinline__ void interp_k0(const K4Dev& s, const float w[8], cons
     }
 }
 
+// The same gather for a copy of exactly NQ channel quads per voxel (s.Cpad == 4 * NQ, the wgmma marchers' configs):
+// no run-time channel count and no branch per quad, the corner rows addressed once with the quads at immediate offsets,
+// loads issued KR corners (all their quads) at a time.  ptxas still interleaves the loads of later corners with the
+// FMAs of earlier ones; what this saves is the per-quad branches and address arithmetic.  With 4 quads the unbranched
+// loads raise the register pressure at the marchers' 128-register cap (config 4 would spill 76 bytes, not 28), so
+// those configs keep the per-quad rounds of interp_k0.  Per channel the same products and FMA order as interp_k0.
+template <int NQ, int KR = 2>
+__device__ __forceinline__ void interp_k0_cfg(const K4Dev& s, const float w[8], const int idx[8], float* out) {
+    static_assert(8 % KR == 0, "corners per round");
+    if (NQ > 3) {
+        interp_k0<NQ>(s, w, idx, out);
+        return;
+    }
+    const float4* base = reinterpret_cast<const float4*>(s.k0cl);
+    float4 a[NQ];
+#pragma unroll
+    for (int k0 = 0; k0 < 8; k0 += KR) {
+        float4 v[KR][NQ];
+#pragma unroll
+        for (int k = 0; k < KR; ++k) {
+            const float4* p = base + (size_t)idx[k0 + k] * NQ;
+#pragma unroll
+            for (int j = 0; j < NQ; ++j) v[k][j] = __ldg(p + j);
+        }
+#pragma unroll
+        for (int j = 0; j < NQ; ++j)
+#pragma unroll
+            for (int k = 0; k < KR; ++k) {
+                const float wk = w[k0 + k];
+                if (k0 + k == 0) {                      // out_acc = 0 + v*w: the FMA with 0 is the product
+                    a[j].x = __fmul_rn(v[k][j].x, wk); a[j].y = __fmul_rn(v[k][j].y, wk);
+                    a[j].z = __fmul_rn(v[k][j].z, wk); a[j].w = __fmul_rn(v[k][j].w, wk);
+                } else {
+                    a[j].x = __fmaf_rn(v[k][j].x, wk, a[j].x); a[j].y = __fmaf_rn(v[k][j].y, wk, a[j].y);
+                    a[j].z = __fmaf_rn(v[k][j].z, wk, a[j].z); a[j].w = __fmaf_rn(v[k][j].w, wk, a[j].w);
+                }
+            }
+    }
+#pragma unroll
+    for (int j = 0; j < NQ; ++j) {
+        out[4 * j + 0] = a[j].x; out[4 * j + 1] = a[j].y; out[4 * j + 2] = a[j].z; out[4 * j + 3] = a[j].w;
+    }
+}
+
 // ---------------------------------------------------------------------------------------------
 // Empty-space skipping (result preserving).  Called for a sample at step i that is inside the bounding box, maps to
 // occupancy voxel (mi, mj, mk) and found it EMPTY.  s.skip holds, per cell of K4_SKIP_B^3 occupancy voxels, the

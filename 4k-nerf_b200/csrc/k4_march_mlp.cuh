@@ -64,23 +64,69 @@ struct PhaseClock {
     }
 };
 
+// What the epilogue needs of a lane's two rows of a 64-row half (rows g and g + 8 of its warp's 16): channel t's logit
+// (o[0] / o[2] of the m64n16 accumulator, diffuse term added), the sample weight and the owning ray; owner -1 for a row
+// beyond `valid` and for lane t == 3, which has no channel.
+struct MlpEpiRows {
+    float logit[2], w[2];
+    int owner[2];
+};
+
+template <bool DIRECT>
+__device__ __forceinline__ MlpEpiRows mlp_epi_rows(const float (&o)[8], int row0, int valid, unsigned slot0, const float* qw,
+                                                   const unsigned char* qowner, const float* qdiff, int t) {
+    MlpEpiRows e;
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+        const int row = row0 + 8 * rr;
+        e.logit[rr] = o[2 * rr];
+        e.w[rr] = 0.f;
+        e.owner[rr] = -1;
+        if (t < 3 && row < valid) {
+            const unsigned slot = slot0 + (unsigned)row;
+            if (!DIRECT) e.logit[rr] = __fadd_rn(e.logit[rr], qdiff[slot * 3 + t]);      // rgb_logit + k0_diffuse
+            e.w[rr] = qw[slot];
+            e.owner[rr] = qowner[slot];
+        }
+    }
+    return e;
+}
+
+// w * sigmoid(logit) of the rows, added to racc[3 * owner + t].  A shared-memory float atomicAdd is a compare-and-swap
+// loop on sm_90; per-warp accumulator slices with plain adds and a same-owner check instead measured 1 % slower per
+// frame, so the atomics stay.
+__device__ __forceinline__ void mlp_epilogue(const MlpEpiRows& e, float* racc, int t) {
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr)
+        if (e.owner[rr] >= 0) atomicAdd(racc + e.owner[rr] * 3 + t, e.w[rr] * sigmoid_ref(e.logit[rr]));
+}
+
 // Rows [0, valid) of the ring tile at shared address a_tile (canonical K-major, KPAD/8 chunks per row).  Row r is
 // queue slot slot0 + r: its colour, weighted by qw[slot], is added to racc[3 * qowner[slot] + c].  Called by all 128
-// threads of one warpgroup (wt = thread index in the group); `valid` must be the same for all of them.  `mark` receives
-// the phase boundaries (PhaseClock).
-template <int W, int KPAD, bool DIRECT, class Mark = NoPhases>
+// threads of one warpgroup (wt = thread index in the group); `valid` must be the same for all of them.
+//
+// consumed() is called once by every thread when the batch's ring rows and queue slots may be reused: after the last
+// L3 has retired and the last half's epilogue inputs are in registers.  That epilogue runs after it, while the marchers
+// already fill the ring, unless colour_first is set; then consumed() also means "colours accumulated".  Running the
+// first half's epilogue under the second half's L1 MMAs instead keeps the accumulator, the epilogue and its inputs
+// live at once: the 128-wide configurations then need 150 registers of the 128 and ptxas serialises the wgmmas (C7518).
+// `mark` receives the phase boundaries (PhaseClock).
+template <int W, int KPAD, bool DIRECT, class Consumed, class Mark = NoPhases>
 __device__ __forceinline__ void mlp_batch_wgmma(uint32_t a_tile, const unsigned char* blob, const TcBlobLayout& BL, int valid,
                                                 unsigned slot0, const float* qw, const unsigned char* qowner, const float* qdiff,
-                                                float* racc, int wt, const Mark& mark = Mark()) {
+                                                float* racc, int wt, const Consumed& consumed, bool colour_first,
+                                                const Mark& mark = Mark()) {
     constexpr int KCH = KPAD / 8, KCHW = W / 8, NC = W / 64;      // NC: 64-column blocks of a hidden layer
     static_assert(W % 64 == 0, "hidden width");
-    const int warp = wt >> 5, lane = wt & 31, g = lane >> 2, t = lane & 3;
+    const int warp = wt >> 5, g = (wt & 31) >> 2, t = wt & 3;
     const uint32_t blob_s = (uint32_t)__cvta_generic_to_shared(blob);
     const uint32_t w1 = blob_s + BL.off_w1, w2 = blob_s + BL.off_w2, w3 = blob_s + BL.off_w3;
     const uint32_t b1 = blob_s + BL.off_b1, b2 = blob_s + BL.off_b2, b3 = blob_s + BL.off_b3, ones = blob_s + BL.off_ones;
     const uint64_t d_ones = wg_desc(ones, 128, 256);
+    const int halves = valid > 64 ? 2 : (valid > 0 ? 1 : 0);
+    MlpEpiRows pend;                                    // the last half's epilogue inputs
 #pragma unroll 1
-    for (int mh = 0; mh < 2 && mh * 64 < valid; ++mh) {
+    for (int mh = 0; mh < halves; ++mh) {
         const uint32_t a_half = a_tile + mh * 8 * KCH * 128;
         uint32_t h1[W / 16][4], h2[W / 16][4];
         // L1 and L2 each run as ONE chain over all W output columns.  Splitting them into 64-column chains that differ
@@ -125,19 +171,17 @@ __device__ __forceinline__ void mlp_batch_wgmma(uint32_t a_tile, const unsigned 
         wg_fence_acc(o);
         mark(K4_PH_L_L3);
         // W3 / B3 hold output channel c in column 2c (k4_scene_create), so channel c of rows g / g+8 is o[0] / o[2] of lane
-        // t = c: three lanes of each quad share the epilogue, two sigmoids and two atomics each
-        if (t < 3) {
-#pragma unroll
-            for (int rr = 0; rr < 2; ++rr) {
-                const int row = mh * 64 + warp * 16 + g + 8 * rr;
-                if (row < valid) {
-                    const unsigned slot = slot0 + (unsigned)row;
-                    float logit = o[2 * rr];
-                    if (!DIRECT) logit = __fadd_rn(logit, qdiff[slot * 3 + t]);      // rgb_logit + k0_diffuse
-                    atomicAdd(racc + qowner[slot] * 3 + t, qw[slot] * sigmoid_ref(logit));
-                }
-            }
+        // t = c: three lanes of each quad share the epilogue
+        pend = mlp_epi_rows<DIRECT>(o, mh * 64 + warp * 16 + g, valid, slot0, qw, qowner, qdiff, t);
+        if (mh + 1 < halves) {
+            mlp_epilogue(pend, racc, t);
+            mark(K4_PH_L_EPILOGUE);
         }
+    }
+    if (!colour_first) consumed();
+    if (halves > 0) {
+        mlp_epilogue(pend, racc, t);
         mark(K4_PH_L_EPILOGUE);
     }
+    if (colour_first) consumed();
 }

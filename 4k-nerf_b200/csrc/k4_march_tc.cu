@@ -131,7 +131,7 @@ k4_march_tc_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
         asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");      // generic smem writes -> async proxy
         wg_bar(wg);
         if (wt == 0) ++n_batches;
-        mlp_batch_wgmma<W, KPAD, true>(a_tile, blob, BL, valid, head & (TC_RING - 1), qw, qowner, nullptr, racc, wt);
+        mlp_batch_wgmma<W, KPAD, true>(a_tile, blob, BL, valid, head & (TC_RING - 1), qw, qowner, nullptr, racc, wt, [] {}, true);
     };
 
     for (unsigned iter = 0;; ++iter) {
@@ -282,7 +282,7 @@ k4_march_tc_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
                     if (shade) {
                         const unsigned slot = (base + __popc(bal & ((1u << lane) - 1u))) & (TC_RING - 1);
                         float f[Cfg::NS];
-                        interp_k0<Cfg::CPAD / 4>(s, cw, cidx, f);       // f[0..C) (CPAD >= C; extra lanes unused)
+                        interp_k0_cfg<Cfg::CPAD / 4>(s, cw, cidx, f);       // f[0..C) (CPAD >= C; extra lanes unused)
                         if (Cfg::KIND == K4_KIND_DMPIGO) {
                             const float pe[3] = {cell.cz, cell.cy, cell.cx};
                             f[Cfg::C + 0] = pe[0]; f[Cfg::C + 1] = pe[1]; f[Cfg::C + 2] = pe[2];
@@ -382,7 +382,7 @@ template <class Cfg>
 bool matches(const K4Dev& v) {
     return v.kind == Cfg::KIND && v.C == Cfg::C && v.viewpe == Cfg::VIEWPE && v.width == Cfg::W && v.depth == 3 &&
            v.dim0 == Cfg::DIM0 && (Cfg::KIND == K4_KIND_DMPIGO ? v.spape == Cfg::SPAPE : v.direct != 0) &&
-           v.tc_blob != nullptr && v.tc_kpad == Cfg::KPAD && v.tc_exact != 0;
+           v.tc_blob != nullptr && v.tc_kpad == Cfg::KPAD && v.tc_exact != 0 && v.Cpad == Cfg::CPAD;
 }
 
 }  // namespace

@@ -10,9 +10,11 @@
 //             Back-pressure: batch B may only be submitted once batch B-1 has been consumed (DONE
 //             mbarrier), so one batch per marcher group is in flight while the next one fills.
 //   WG2, WG3  MLP, one group per marcher slot: wait FULL -> the three layers as warpgroup MMAs with
-//             register-resident activations (mlp_batch_wgmma, k4_march_mlp.cuh), colours accumulated
-//             into the owning rays -> arrive DONE.  The two MLP groups and the two marcher groups all
-//             run concurrently, so gathers, epilogues and MMAs of different batches overlap.
+//             register-resident activations (mlp_batch_wgmma, k4_march_mlp.cuh) -> arrive DONE once the
+//             batch's rows and queue slots are read -> colours accumulated into the owning rays while the
+//             marchers refill the ring.  A ray tile's last batch arrives on DONE only after its colours
+//             (WgCtl::last), since the marchers read them next.  The two MLP groups and the two marcher
+//             groups all run concurrently, so gathers, epilogues and MMAs of different batches overlap.
 // Arithmetic is identical to k4_march_tc.cu (same rows, same MMAs, same epilogues).
 #include "k4_internal.cuh"
 #include "k4_march_common.cuh"
@@ -54,11 +56,13 @@ struct TcCfg {
     static constexpr int WG_RACC = WG_QW + TC_RING * 4;      // float[128*3]
     static constexpr int WG_OWNER = WG_RACC + 128 * 3 * 4;   // u8[384]
     static constexpr int WG_QDIFF = WG_OWNER + TC_RING;      // float[384*3]: diffuse logits of the queued samples (!DIRECT only)
-    static constexpr int WG_MISC = WG_QDIFF + (DIRECT ? 0 : TC_RING * 3 * 4);   // tail, tile slots, valid counts, exit flag, mbarriers
+    static constexpr int WG_VW = WG_QDIFF + (DIRECT ? 0 : TC_RING * 3 * 4);     // u32[NVW][128]: packed view embedding per ray
+    static constexpr int WG_MISC = WG_VW + NVW * 128 * 4;    // tail, tile slots, valid counts, exit flag, mbarriers
     static constexpr int WG_BYTES = (WG_MISC + 128 + 1023) & ~1023;
     static constexpr int CTA_MISC = BLOB_PAD + 2 * WG_BYTES; // weight mbarrier
     static constexpr int SMEM = CTA_MISC + 64;
     static constexpr int PROF_SMEM = SMEM + 4 * PhaseClock::WORDS * 8;   // + the phase counters of the profiled kernel
+    static_assert(PROF_SMEM <= 227 * 1024, "shared memory of one block");
 };
 
 __device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -108,9 +112,10 @@ struct WgCtl {
     unsigned int exit_flag;        // set when the group has no more tiles
     long long tile_slot[2];
     int valid[TC_TILES];           // real rows of the batch in each ring tile
-    int pad;
+    int last[TC_TILES];            // the batch is its ray tile's last: DONE only once its colours are accumulated
     uint64_t full_bar;             // marcher -> MLP: a batch is complete            (count 1)
-    uint64_t done_bar;             // MLP -> marcher: a batch has been consumed      (count 128)
+    uint64_t done_bar;             // MLP -> marcher: a batch's rows and queue slots are free, and for a tile's last
+                                   // batch its colours are accumulated                (count 128)
 };
 
 // PROF: the profiled instantiation (k4_testing_march_phases).  It adds the phase marks of PhaseClock and nothing else, and
@@ -168,6 +173,7 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
         uint32_t full_ph = 0;
         unsigned nb = 0;
         unsigned long long n_batches = 0;
+        auto consumed = [&] { mbar_arrive(&c->done_bar); };      // 128 arrivals = DONE
         for (;;) {
             tc_mbar_wait(&c->full_bar, full_ph); full_ph ^= 1;
             mark(K4_PH_L_WAIT_FULL);
@@ -175,13 +181,13 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
             const unsigned tile = nb % TC_TILES;
             if (wt == 0) ++n_batches;
             const int valid = *reinterpret_cast<volatile int*>(&c->valid[tile]);
+            const bool last = *reinterpret_cast<volatile int*>(&c->last[tile]) != 0;
             if (PROF)
                 mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0>(ring_s + tile * Cfg::TILE_BYTES, blob, BL, valid, tile * 128u, qw, qowner,
-                                                           qdiff, racc, wt, clk);
+                                                           qdiff, racc, wt, consumed, last, clk);
             else
                 mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0>(ring_s + tile * Cfg::TILE_BYTES, blob, BL, valid, tile * 128u, qw, qowner,
-                                                           qdiff, racc, wt);
-            mbar_arrive(&c->done_bar);              // 128 arrivals = batch consumed
+                                                           qdiff, racc, wt, consumed, last);
             ++nb;
         }
         if (rp.counters && wt == 0) atomicAdd(rp.counters + 3, n_batches);
@@ -196,6 +202,7 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
         float* racc = reinterpret_cast<float*>(wgb + Cfg::WG_RACC);
         unsigned char* qowner = wgb + Cfg::WG_OWNER;
         float* qdiff = reinterpret_cast<float*>(wgb + Cfg::WG_QDIFF);
+        uint32_t* vws = reinterpret_cast<uint32_t*>(wgb + Cfg::WG_VW) + wt;     // this ray's words at a stride of 128
         WgCtl* ctl = wg_ctl(wg);
         volatile unsigned int* tailp = &ctl->tail;
         volatile long long* tile_slot = ctl->tile_slot;
@@ -212,7 +219,10 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
         // group keeps marching into the next tile(s) while its outstanding batch is in the MLP group;
         // with 3 ring tiles the rows of batches B+1 (filling) and B+2 (overflow of a step) never
         // alias the tile of the outstanding batch B.
-        auto submit = [&](int valid) {
+        // `last`: no more rows of this ray tile follow, so the MLP group arrives on DONE only after the batch's
+        // colours are in racc (other batches arrive as soon as their rows are read, before their epilogue).
+        bool tile_open = false;            // a batch of this ray tile was submitted without `last`
+        auto submit = [&](int valid, bool last) {
             asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");      // generic smem writes -> async proxy
             named_bar(wg + 1);
             mark(K4_PH_M_RENDEZVOUS);
@@ -220,11 +230,13 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
             mark(K4_PH_M_WAIT_DONE);
             if (wt == 0) {
                 *reinterpret_cast<volatile int*>(&ctl->valid[n_sub % TC_TILES]) = valid;
+                *reinterpret_cast<volatile int*>(&ctl->last[n_sub % TC_TILES]) = last ? 1 : 0;
                 __threadfence_block();
                 mbar_arrive(&ctl->full_bar);
             }
             ++n_sub;
             head += 128u;
+            tile_open = !last;
         };
 
         for (unsigned iter = 0;; ++iter) {
@@ -302,6 +314,9 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
 #pragma unroll
                 for (int j = 0; j < Cfg::NVW; ++j) vw[j] = pack2(ve[2 * j], ve[2 * j + 1]);
             }
+            // kept in shared memory while marching, where it would hold NVW registers of the capped 128 for the whole tile
+#pragma unroll
+            for (int j = 0; j < Cfg::NVW; ++j) vws[j * 128] = vw[j];
 
             mark(K4_PH_M_SETUP);
             float T = 1.f, acc_depth = 0.f;
@@ -420,7 +435,7 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
                         if (shade) {
                             const unsigned slot = (base + __popc(bal & ((1u << lane) - 1u))) % (unsigned)TC_RING;
                             float f[Cfg::NF];
-                            interp_k0<Cfg::CPAD / 4>(s, cw, cidx, f);
+                            interp_k0_cfg<Cfg::CPAD / 4>(s, cw, cidx, f);
                             if (Cfg::KIND == K4_KIND_DMPIGO) {
                                 const float pe[3] = {cell.cz, cell.cy, cell.cx};
                                 f[Cfg::C + 0] = pe[0]; f[Cfg::C + 1] = pe[1]; f[Cfg::C + 2] = pe[2];
@@ -434,18 +449,20 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
                                     }
                             }
                             if (Cfg::NS0 & 1) f[Cfg::K0OFF + Cfg::NS0] = 0.f;          // pad column of an odd feature count
-                            uint32_t row[KPAD / 2];
-#pragma unroll
-                            for (int j = 0; j < KPAD / 2; ++j) {
-                                if (j < Cfg::NS / 2) row[j] = pack2(f[Cfg::K0OFF + 2 * j], f[Cfg::K0OFF + 2 * j + 1]);
-                                else if (j < Cfg::NS / 2 + Cfg::NVW) row[j] = vw[j - Cfg::NS / 2];
-                                else row[j] = 0u;
-                            }
                             unsigned char* rowp = aring + (slot >> 7) * Cfg::TILE_BYTES + tc_canon_off((int)(slot & 127), 0, KCH);
 #pragma unroll
-                            for (int kc = 0; kc < KCH; ++kc)
-                                if (kc * 4 < Cfg::NS / 2 + Cfg::NVW)
-                                    *reinterpret_cast<uint4*>(rowp + kc * 128) = make_uint4(row[4 * kc], row[4 * kc + 1], row[4 * kc + 2], row[4 * kc + 3]);
+                            for (int kc = 0; kc < KCH; ++kc) {
+                                if (kc * 4 >= Cfg::NS / 2 + Cfg::NVW) break;           // chunks that are all padding stay zero
+                                uint32_t q[4];
+#pragma unroll
+                                for (int e = 0; e < 4; ++e) {
+                                    const int j = 4 * kc + e;
+                                    if (j < Cfg::NS / 2) q[e] = pack2(f[Cfg::K0OFF + 2 * j], f[Cfg::K0OFF + 2 * j + 1]);
+                                    else if (j < Cfg::NS / 2 + Cfg::NVW) q[e] = vws[(j - Cfg::NS / 2) * 128];
+                                    else q[e] = 0u;
+                                }
+                                *reinterpret_cast<uint4*>(rowp + kc * 128) = make_uint4(q[0], q[1], q[2], q[3]);
+                            }
                             qw[slot] = w_sample;
                             qowner[slot] = (unsigned char)wt;
                             if (!Cfg::DIRECT) { qdiff[slot * 3 + 0] = f[0]; qdiff[slot * 3 + 1] = f[1]; qdiff[slot * 3 + 2] = f[2]; }
@@ -458,10 +475,10 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
                 mark(K4_PH_M_RENDEZVOUS);
                 const unsigned tail = *tailp;                          // stable until the next barrier
                 if (tail - head >= 128u) {
-                    submit(128);
+                    submit(128, !live && tail - head == 128u);
                 } else if (!live) {
-                    if (tail != head) {
-                        submit((int)(tail - head));
+                    if (tail != head || tile_open) {                   // without rows the tile's last batch only carries `last`
+                        submit((int)(tail - head), true);
                         named_bar(wg + 1);                             // everyone has read `tail`
                         if (wt == 0) *tailp = head;
                         mark(K4_PH_M_RENDEZVOUS);
@@ -513,6 +530,7 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
 // phases: NULL for the production kernel, else the profiled one writes there (room for max_ctas CTAs); *n_ctas: CTAs launched
 template <class Cfg>
 int launch_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st, unsigned long long* phases, int max_ctas, int* n_ctas) {
+    if (sc->dev.Cpad != Cfg::CPAD) return K4_ERR_UNSUPPORTED;     // the k0 gather's stride is the config's
     auto kern = phases ? k4_march_ws_kernel<Cfg, true> : k4_march_ws_kernel<Cfg, false>;
     const int smem = phases ? Cfg::PROF_SMEM : Cfg::SMEM;
     int dev = 0, sms = 0;
@@ -583,7 +601,7 @@ k4_test_rgbnet_ws_kernel(const __grid_constant__ K4Dev s, const float* __restric
     asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");      // generic smem writes -> async proxy
     tc_mbar_wait(bar, 0);
     __syncthreads();
-    mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0>(s_u32(tile), blob, BL, valid, 0u, qw, qowner, qdiff, racc, wt);
+    mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0>(s_u32(tile), blob, BL, valid, 0u, qw, qowner, qdiff, racc, wt, [] {}, true);
     __syncthreads();
 #pragma unroll
     for (int c = 0; c < 3; ++c) racc_out[3 * (r0 + wt) + c] = racc[3 * wt + c];
