@@ -9,7 +9,10 @@
 //       its epilogue (epilogue_sft);
 //   sft_mma_kernel<COUT>   SFTLayer (lib/sr_esrnet.py:112-123) as its own pass (K4_SR_FUSE_SFT=0), mma.sync on the
 //       same operand fragments as the fused epilogue; sft_kernel is its fp32 one-thread-per-pixel form (K4_SFT_FP32=1);
-//   condnet_kernel         CondNet (lib/sr_esrnet.py:440-444), one thread per pixel, fp32.
+//   condnet_mma_kernel     CondNet (lib/sr_esrnet.py:440-444) of the depth condition (num_cond 1) on mma.sync, fp32-class
+//       through a 3-term fp16 split; condnet_wide_mma_kernel<NKS> the same for a wide condition (num_cond 2..64: the
+//       view-direction embedding), whose 3x3 layer is an implicit GEMM on the tensor cores as well;
+//   condnet_kernel<WIDE>   CondNet, one thread per pixel, fp32 (the A/B reference, K4_CONDNET_FP32=1).
 //
 // Numerics: conv operands are fp16 (weights and activations), accumulation fp32, the residual trunk and all CondNet
 // math stay fp32.  (The reference itself runs these convs with TF32 operands: torch.backends.cudnn.allow_tf32
@@ -773,13 +776,18 @@ __global__ void pack_sft_frag_kernel(const float* __restrict__ w, unsigned char*
     if (i < cout) { reinterpret_cast<float*>(dst + L.off_b1s)[i] = s1b[i] + 1.f; reinterpret_cast<float*>(dst + L.off_b1h)[i] = h1b[i]; }
 }
 
-// CondNet: conv3x3(1->64) lrelu, 1x1 64->64 lrelu, 1x1 64->64 lrelu, 1x1 64->32   (lib/sr_esrnet.py:440-444)
-struct CondParams { const float* cond_in; const float* w; float* cond_out; int H, W; int y_lo, y_hi; __half* cond16; };   // w: c0 [64][9], b0[64], c2 [64][64], b2, c4 [64][64], b4, c6 [32][64], b6
+// CondNet: conv3x3(num_cond->64) lrelu, 1x1 64->64 lrelu, 1x1 64->64 lrelu, 1x1 64->32   (lib/sr_esrnet.py:440-444)
+// cond_in: planar fp32 [nc][H][W].  w: c0 [64][nc][9], b0[64], c2 [64][64], b2, c4 [64][64], b4, c6 [32][64], b6
+struct CondParams { const float* cond_in; const float* w; float* cond_out; int H, W; int y_lo, y_hi; __half* cond16; int nc; };
 
+// WIDE (nc > 1, the view-conditioned decoder): layer 0 runs channel by channel with its weights read from global memory
+// (64 x nc x 9 floats, 147 KB at nc = 64); shared memory holds the 1x1 layers and every bias at the offsets of nc = 1.
+template <bool WIDE>
 __global__ void __launch_bounds__(128) condnet_kernel(const __grid_constant__ CondParams p) {
     constexpr int NW = 64 * 9 + 64 + 2 * (64 * 64 + 64) + 32 * 64 + 32;
     extern __shared__ __align__(16) float sw[];
-    for (int i = threadIdx.x; i < NW; i += blockDim.x) sw[i] = __ldg(p.w + i);
+    const long long wskip = WIDE ? 576LL * (p.nc - 1) : 0;            // block offset of b0 minus that of nc = 1
+    for (int i = threadIdx.x + (WIDE ? 576 : 0); i < NW; i += blockDim.x) sw[i] = __ldg(p.w + wskip + i);
     __syncthreads();
     const float* c0 = sw; const float* b0 = c0 + 576; const float* c2 = b0 + 64; const float* b2 = c2 + 4096;
     const float* c4 = b2 + 64; const float* b4 = c4 + 4096; const float* c6 = b4 + 64; const float* b6 = c6 + 2048;
@@ -787,21 +795,46 @@ __global__ void __launch_bounds__(128) condnet_kernel(const __grid_constant__ Co
     const long long pix = (long long)p.y_lo * p.W + (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (pix >= (long long)p.y_hi * p.W) return;
     const int y = (int)(pix / p.W), x = (int)(pix - (long long)y * p.W);
-    float n[9];
-#pragma unroll
-    for (int dy = 0; dy < 3; ++dy)
-#pragma unroll
-        for (int dx = 0; dx < 3; ++dx) {
-            const int yy = y + dy - 1, xx = x + dx - 1;
-            n[dy * 3 + dx] = (yy >= 0 && yy < p.H && xx >= 0 && xx < p.W) ? __ldg(p.cond_in + (size_t)yy * p.W + xx) : 0.f;
-        }
     float a[64], b[64];
-#pragma unroll 4
-    for (int o = 0; o < 64; ++o) {
-        float v = b0[o];
+    if constexpr (WIDE) {
+        // same FMA order per output as below: from the bias, channel by channel, taps in row-major order
 #pragma unroll
-        for (int k = 0; k < 9; ++k) v = fmaf(c0[o * 9 + k], n[k], v);
-        a[o] = v > 0.f ? v : 0.2f * v;
+        for (int o = 0; o < 64; ++o) a[o] = b0[o];
+        const long long plane = (long long)p.H * p.W;
+#pragma unroll 1
+        for (int ci = 0; ci < p.nc; ++ci) {
+            float n[9];
+#pragma unroll
+            for (int dy = 0; dy < 3; ++dy)
+#pragma unroll
+                for (int dx = 0; dx < 3; ++dx) {
+                    const int yy = y + dy - 1, xx = x + dx - 1;
+                    n[dy * 3 + dx] = (yy >= 0 && yy < p.H && xx >= 0 && xx < p.W) ? __ldg(p.cond_in + ci * plane + (size_t)yy * p.W + xx) : 0.f;
+                }
+            const float* w0 = p.w + ci * 9;
+#pragma unroll
+            for (int o = 0; o < 64; ++o)
+#pragma unroll
+                for (int k = 0; k < 9; ++k) a[o] = fmaf(__ldg(w0 + (size_t)o * p.nc * 9 + k), n[k], a[o]);
+        }
+#pragma unroll
+        for (int o = 0; o < 64; ++o) a[o] = a[o] > 0.f ? a[o] : 0.2f * a[o];
+    } else {
+        float n[9];
+#pragma unroll
+        for (int dy = 0; dy < 3; ++dy)
+#pragma unroll
+            for (int dx = 0; dx < 3; ++dx) {
+                const int yy = y + dy - 1, xx = x + dx - 1;
+                n[dy * 3 + dx] = (yy >= 0 && yy < p.H && xx >= 0 && xx < p.W) ? __ldg(p.cond_in + (size_t)yy * p.W + xx) : 0.f;
+            }
+#pragma unroll 4
+        for (int o = 0; o < 64; ++o) {
+            float v = b0[o];
+#pragma unroll
+            for (int k = 0; k < 9; ++k) v = fmaf(c0[o * 9 + k], n[k], v);
+            a[o] = v > 0.f ? v : 0.2f * v;
+        }
     }
 #pragma unroll 2
     for (int o = 0; o < 64; ++o) {
@@ -845,10 +878,11 @@ __host__ __device__ inline CnmLayout cnm_layout() {
     L.total = (o + 15) & ~15;
     return L;
 }
-// w: c0 [64][9], b0[64], c2 [64][64], b2, c4 [64][64], b4, c6 [32][64], b6  (the fp32 kernel's packing)
-__global__ void pack_condnet_mma_kernel(const float* __restrict__ w, unsigned char* __restrict__ dst) {
+// w: c0 [64][nc][9], b0[64], c2 [64][64], b2, c4 [64][64], b4, c6 [32][64], b6  (the fp32 kernel's packing).  The fp32
+// layer-0 weights w0 are packed at nc = 1 only; a wide layer 0 is packed by pack_condnet_wide_kernel.
+__global__ void pack_condnet_mma_kernel(const float* __restrict__ w, int nc, unsigned char* __restrict__ dst) {
     const CnmLayout L = cnm_layout();
-    const float* c0 = w; const float* b0 = c0 + 576; const float* c2 = b0 + 64; const float* b2 = c2 + 4096;
+    const float* c0 = w; const float* b0 = c0 + 576 * nc; const float* c2 = b0 + 64; const float* b2 = c2 + 4096;
     const float* c4 = b2 + 64; const float* b4 = c4 + 4096; const float* c6 = b4 + 64; const float* b6 = c6 + 2048;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     auto split = [&](int offh, int offl, int n, int k, float v) {
@@ -858,12 +892,31 @@ __global__ void pack_condnet_mma_kernel(const float* __restrict__ w, unsigned ch
     };
     if (i < 4096) { split(L.w1h, L.w1l, i >> 6, i & 63, c2[i]); split(L.w2h, L.w2l, i >> 6, i & 63, c4[i]); }
     if (i < 2048) split(L.w3h, L.w3l, i >> 6, i & 63, c6[i]);
-    if (i < 576) reinterpret_cast<float*>(dst + L.w0)[i] = c0[i];
+    if (i < 576 && nc == 1) reinterpret_cast<float*>(dst + L.w0)[i] = c0[i];
     if (i < 64) { reinterpret_cast<float*>(dst + L.b0)[i] = b0[i]; reinterpret_cast<float*>(dst + L.b1)[i] = b2[i]; reinterpret_cast<float*>(dst + L.b2)[i] = b4[i]; }
     if (i < 32) reinterpret_cast<float*>(dst + L.b3)[i] = b6[i];
 }
 
-struct CondMmaParams { const float* cond_in; const unsigned char* wblk; float* cond_out; __half* cond16; int H, W, y_lo, y_hi; };
+// Wide layer 0 (1 < nc <= 64): an implicit GEMM with K = 9 taps x 64 channels, tap-major.  Its weights follow the
+// cnm_layout block as hi / lo fp16 rows [n][tap * 64 + c], CNW_PITCH halfs apart (584 = 4 words mod 32 banks: the eight
+// rows g and four column pairs tq of a B-fragment load hit 32 different banks).  Channels c >= nc are zero.
+constexpr int CNW_PITCH = 9 * 64 + 8;
+__host__ __device__ inline int cnw_bytes() { return cnm_layout().total + 2 * 64 * CNW_PITCH * 2; }
+
+// c0: CondNet.0 [64][nc][3][3] fp32 -> the hi / lo rows behind the cnm_layout block of dst (zeroed beforehand)
+__global__ void pack_condnet_wide_kernel(const float* __restrict__ c0, int nc, unsigned char* __restrict__ dst) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 64 * 9 * nc) return;
+    const int n = i / (9 * nc), r = i - n * 9 * nc, c = r / 9, t = r - c * 9;
+    __half* wh = reinterpret_cast<__half*>(dst + cnm_layout().total);
+    __half* wl = wh + 64 * CNW_PITCH;
+    const __half hi = __float2half_rn(c0[i]);
+    wh[n * CNW_PITCH + t * 64 + c] = hi;
+    wl[n * CNW_PITCH + t * 64 + c] = __float2half_rn(c0[i] - __half2float(hi));
+}
+
+// cond_in: planar fp32 [nc][H][W]; wblk: the cnm_layout block (+ the wide layer-0 rows when nc > 1)
+struct CondMmaParams { const float* cond_in; const unsigned char* wblk; float* cond_out; __half* cond16; int H, W, y_lo, y_hi, nc; };
 
 // accumulator fragments of 2 adjacent n8 blocks -> hi / lo A fragments of one k16 step.  Both halves saturate: beyond
 // the fp16 range hi = +-65504 and lo = x - hi, itself clamped, so an activation of 65520 or more stays finite (a
@@ -895,6 +948,41 @@ __device__ __forceinline__ void cnm_layer(const unsigned char* sm, int offh, int
             sr_hmma(c[j], al[ks], bh0, bh1);                     // small terms first
             sr_hmma(c[j], ah[ks], *reinterpret_cast<const uint32_t*>(wl), *reinterpret_cast<const uint32_t*>(wl + 8));
             sr_hmma(c[j], ah[ks], bh0, bh1);
+        }
+    }
+}
+
+// CondNet's 1x1 layers (64 -> 64, 64 -> 64, 64 -> 32) on layer 0's split LeakyReLU output, and the cond_out / cond16
+// stores of the block's two pixel rows
+__device__ __forceinline__ void cnm_tail(const unsigned char* csm, const CnmLayout& L, uint32_t (&ah)[4][4], uint32_t (&al)[4][4],
+                                         int g, int tq, const CondMmaParams& p, long long pixA, long long pixB, bool inA, bool inB) {
+    float c[8][4];
+    cnm_layer<8>(csm, L.w1h, L.w1l, L.b1, ah, al, g, tq, c);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) c[j][e] = fmaxf(c[j][e], 0.2f * c[j][e]);
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) cnm_split_frag(c[2 * ks], c[2 * ks + 1], ah[ks], al[ks]);
+    cnm_layer<8>(csm, L.w2h, L.w2l, L.b2, ah, al, g, tq, c);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) c[j][e] = fmaxf(c[j][e], 0.2f * c[j][e]);
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) cnm_split_frag(c[2 * ks], c[2 * ks + 1], ah[ks], al[ks]);
+    float o[4][4];
+    cnm_layer<4>(csm, L.w3h, L.w3l, L.b3, ah, al, g, tq, o);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int ch = 8 * j + 2 * tq;
+        if (inA) {
+            *reinterpret_cast<float2*>(p.cond_out + pixA * 32 + ch) = make_float2(o[j][0], o[j][1]);
+            if (p.cond16) *reinterpret_cast<__half2*>(p.cond16 + pixA * 32 + ch) = sr_h2sat(o[j][0], o[j][1]);
+        }
+        if (inB) {
+            *reinterpret_cast<float2*>(p.cond_out + pixB * 32 + ch) = make_float2(o[j][2], o[j][3]);
+            if (p.cond16) *reinterpret_cast<__half2*>(p.cond16 + pixB * 32 + ch) = sr_h2sat(o[j][2], o[j][3]);
         }
     }
 }
@@ -944,35 +1032,78 @@ __global__ void __launch_bounds__(128) condnet_mma_kernel(const __grid_constant_
             const float c0[4] = {va[0], va[1], vb[0], vb[1]}, c1[4] = {va[2], va[3], vb[2], vb[3]};
             cnm_split_frag(c0, c1, ah[ks], al[ks]);
         }
+        cnm_tail(csm, L, ah, al, g, tq, p, pixA, pixB, inA, inB);
+    }
+}
+
+// CondNet with a wide condition (1 < nc <= 64, NKS = ceil(nc / 16) k16 steps per tap): layer 0 as an implicit GEMM on
+// the tensor cores, 16-pixel row blocks (M) x 9 taps x 16 NKS channels (K) x 64 outputs (N), with the 3-term split of
+// the 1x1 layers on both operands: the condition is read straight from its planar fp32 map (L1 serves the nine taps'
+// reuse) and split to hi / lo in registers, the weights come pre-split from shared memory.  Channels >= nc and taps
+// outside the map are zero A operands.  The LeakyReLU output feeds the same 1x1 chain as condnet_mma_kernel.
+// Shared memory: the cnm_layout block + 146 KB of layer-0 rows (cnw_bytes, 194 KB): one CTA of 8 warps per SM.
+template <int NKS>
+__global__ void __launch_bounds__(256, 1) condnet_wide_mma_kernel(const __grid_constant__ CondMmaParams p) {
+    extern __shared__ __align__(16) unsigned char csm[];
+    const CnmLayout L = cnm_layout();
+    for (int i = threadIdx.x; i < cnw_bytes() / 16; i += blockDim.x) reinterpret_cast<uint4*>(csm)[i] = __ldg(reinterpret_cast<const uint4*>(p.wblk) + i);
+    __syncthreads();
+    SR_PDL_SYNC();
+    const int lane = threadIdx.x & 31, g = lane >> 2, tq = lane & 3, nwarps = blockDim.x >> 5;
+    const long long p0 = (long long)p.y_lo * p.W, pend = (long long)p.y_hi * p.W;
+    const long long nblk = (pend - p0 + 15) / 16, plane = (long long)p.H * p.W;
+    const __half* W0h = reinterpret_cast<const __half*>(csm + L.total);
+    const __half* W0l = W0h + 64 * CNW_PITCH;
+    const float* B0 = reinterpret_cast<const float*>(csm + L.b0);
+    for (long long blk = (long long)blockIdx.x * nwarps + (threadIdx.x >> 5); blk < nblk; blk += (long long)gridDim.x * nwarps) {
+        const long long pixA = p0 + blk * 16 + g, pixB = pixA + 8;
+        const bool inA = pixA < pend, inB = pixB < pend;
+        const long long pa = inA ? pixA : p0, pb = inB ? pixB : p0;
+        const int ya = (int)(pa / p.W), xa = (int)(pa - (long long)ya * p.W), yb = (int)(pb / p.W), xb = (int)(pb - (long long)yb * p.W);
         float c[8][4];
-        cnm_layer<8>(csm, L.w1h, L.w1l, L.b1, ah, al, g, tq, c);
 #pragma unroll
-        for (int j = 0; j < 8; ++j)
+        for (int j = 0; j < 8; ++j) { c[j][0] = c[j][2] = B0[8 * j + 2 * tq]; c[j][1] = c[j][3] = B0[8 * j + 2 * tq + 1]; }
+#pragma unroll 1
+        for (int t = 0; t < 9; ++t) {
+            const int y1 = ya + t / 3 - 1, x1 = xa + t % 3 - 1, y2 = yb + t / 3 - 1, x2 = xb + t % 3 - 1;
+            const bool okA = y1 >= 0 && y1 < p.H && x1 >= 0 && x1 < p.W, okB = y2 >= 0 && y2 < p.H && x2 >= 0 && x2 < p.W;
+            const float* sA = p.cond_in + (okA ? (long long)y1 * p.W + x1 : 0);
+            const float* sB = p.cond_in + (okB ? (long long)y2 * p.W + x2 : 0);
+            // A operands of the tap's NKS k16 steps: channels 16ks + 2tq, +1 (regs 0 / 1: pixel A / B), +8, +9 (regs 2 / 3)
+            float va[NKS][4], vb[NKS][4];
 #pragma unroll
-            for (int e = 0; e < 4; ++e) c[j][e] = fmaxf(c[j][e], 0.2f * c[j][e]);
+            for (int ks = 0; ks < NKS; ++ks)
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks) cnm_split_frag(c[2 * ks], c[2 * ks + 1], ah[ks], al[ks]);
-        cnm_layer<8>(csm, L.w2h, L.w2l, L.b2, ah, al, g, tq, c);
+                for (int e = 0; e < 4; ++e) {
+                    const int ch = 16 * ks + (e >> 1) * 8 + 2 * tq + (e & 1);
+                    va[ks][e] = (okA && ch < p.nc) ? __ldg(sA + ch * plane) : 0.f;
+                    vb[ks][e] = (okB && ch < p.nc) ? __ldg(sB + ch * plane) : 0.f;
+                }
 #pragma unroll
-        for (int j = 0; j < 8; ++j)
+            for (int ks = 0; ks < NKS; ++ks) {
+                uint32_t ah[4], al[4];
+                const float f0[4] = {va[ks][0], va[ks][1], vb[ks][0], vb[ks][1]}, f1[4] = {va[ks][2], va[ks][3], vb[ks][2], vb[ks][3]};
+                cnm_split_frag(f0, f1, ah, al);
+                const int k0 = t * 64 + 16 * ks + 2 * tq;
 #pragma unroll
-            for (int e = 0; e < 4; ++e) c[j][e] = fmaxf(c[j][e], 0.2f * c[j][e]);
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) cnm_split_frag(c[2 * ks], c[2 * ks + 1], ah[ks], al[ks]);
-        float o[4][4];
-        cnm_layer<4>(csm, L.w3h, L.w3l, L.b3, ah, al, g, tq, o);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int ch = 8 * j + 2 * tq;
-            if (inA) {
-                *reinterpret_cast<float2*>(p.cond_out + pixA * 32 + ch) = make_float2(o[j][0], o[j][1]);
-                if (p.cond16) *reinterpret_cast<__half2*>(p.cond16 + pixA * 32 + ch) = sr_h2sat(o[j][0], o[j][1]);
-            }
-            if (inB) {
-                *reinterpret_cast<float2*>(p.cond_out + pixB * 32 + ch) = make_float2(o[j][2], o[j][3]);
-                if (p.cond16) *reinterpret_cast<__half2*>(p.cond16 + pixB * 32 + ch) = sr_h2sat(o[j][2], o[j][3]);
+                for (int j = 0; j < 8; ++j) {
+                    const __half* wh = W0h + (8 * j + g) * CNW_PITCH + k0;
+                    const __half* wl = W0l + (8 * j + g) * CNW_PITCH + k0;
+                    const uint32_t bh0 = *reinterpret_cast<const uint32_t*>(wh), bh1 = *reinterpret_cast<const uint32_t*>(wh + 8);
+                    sr_hmma(c[j], al, bh0, bh1);                  // small terms first
+                    sr_hmma(c[j], ah, *reinterpret_cast<const uint32_t*>(wl), *reinterpret_cast<const uint32_t*>(wl + 8));
+                    sr_hmma(c[j], ah, bh0, bh1);
+                }
             }
         }
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) c[j][e] = fmaxf(c[j][e], 0.2f * c[j][e]);
+        uint32_t ah[4][4], al[4][4];
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) cnm_split_frag(c[2 * ks], c[2 * ks + 1], ah[ks], al[ks]);
+        cnm_tail(csm, L, ah, al, g, tq, p, pixA, pixB, inA, inB);
     }
 }
 
@@ -1162,19 +1293,23 @@ int make_sft(k4_srnet* n, SrSft& f, const float* const* pw, int cout, cudaStream
     return K4_OK;
 }
 
-// CondNet weights: the 8 tensors of CondNet.0 (64x1x3x3), .2 (64x64), .4 (64x64), .6 (32x64) and their biases -> the fp32
-// block of condnet_kernel and the cnm_layout block of condnet_mma_kernel
-int make_condnet(k4_srnet* n, const float* const* pw, cudaStream_t s) {
-    const size_t nw = 64 * 9 + 64 + 2 * (64 * 64 + 64) + 32 * 64 + 32;
+// CondNet weights: the 8 tensors of CondNet.0 (64 x nc x 3x3), .2 (64x64), .4 (64x64), .6 (32x64) and their biases -> the
+// fp32 block of condnet_kernel and the cnm_layout block of condnet_mma_kernel, followed at nc > 1 by the wide layer-0
+// rows of condnet_wide_mma_kernel
+int make_condnet(k4_srnet* n, const float* const* pw, int nc, cudaStream_t s) {
+    const size_t cnt[8] = {576 * (size_t)nc, 64, 4096, 64, 4096, 64, 2048, 32};
+    size_t nw = 0;
+    for (int q = 0; q < 8; ++q) nw += cnt[q];
     int st = sr_alloc(n, (void**)&n->condnet_w, nw * 4);
     if (st) return st;
     float* dd = n->condnet_w;
-    const size_t cnt[8] = {576, 64, 4096, 64, 4096, 64, 2048, 32};
     for (int q = 0; q < 8; ++q) { cudaMemcpyAsync(dd, pw[q], cnt[q] * 4, cudaMemcpyDeviceToDevice, s); dd += cnt[q]; }
-    st = sr_alloc(n, (void**)&n->condnet_mma, (size_t)cnm_layout().total);
+    const int bytes = nc == 1 ? cnm_layout().total : cnw_bytes();
+    st = sr_alloc(n, (void**)&n->condnet_mma, (size_t)bytes);
     if (st) return st;
-    K4_CUDA_TRY(cudaMemsetAsync(n->condnet_mma, 0, cnm_layout().total, s));
-    pack_condnet_mma_kernel<<<16, 256, 0, s>>>(n->condnet_w, n->condnet_mma);
+    K4_CUDA_TRY(cudaMemsetAsync(n->condnet_mma, 0, bytes, s));
+    pack_condnet_mma_kernel<<<16, 256, 0, s>>>(n->condnet_w, nc, n->condnet_mma);
+    if (nc > 1) pack_condnet_wide_kernel<<<(64 * 9 * nc + 255) / 256, 256, 0, s>>>(n->condnet_w, nc, n->condnet_mma);
     K4_CUDA_TRY(cudaGetLastError());
     return K4_OK;
 }
@@ -1400,20 +1535,45 @@ int run_sft(const SrSft& f, SftParams p, cudaStream_t s, int sel = SRP_AUTO, int
     return f.cout == 64 ? launch_sft_mma<64>(p, f.frag, s) : launch_sft_mma<32>(p, f.frag, s);
 }
 
-// CondNet on rows [y_lo, y_hi) of an h x w condition map: cond32 (fp32 [h*w][32]) and, if given, cond16 (the fp16 operand
-// of the fused SFT epilogues) of those rows.  AUTO reads K4_CONDNET_FP32 per call (fp32 FFMA kernel when it is "1").
+template <int NKS>
+int launch_condnet_wide(const CondMmaParams& cp, cudaStream_t s) {
+    const int smem = cnw_bytes();
+    if (int st = sr_set_smem(condnet_wide_mma_kernel<NKS>, 13 + NKS, smem)) return st;
+    const long long nb = ((long long)(cp.y_hi - cp.y_lo) * cp.W + 15) / 16;
+    long long grid = (nb + 7) / 8;
+    const long long cap = (long long)sr_dev()->sms;                  // one CTA per SM fits its shared memory
+    if (grid > cap) grid = cap;
+    K4_CUDA_TRY(sr_launch(condnet_wide_mma_kernel<NKS>, (unsigned)(grid < 1 ? 1 : grid), 256, (size_t)smem, s, cp));
+    return K4_OK;
+}
+
+// CondNet on rows [y_lo, y_hi) of an h x w condition map (planar fp32 [num_cond][h][w]): cond32 (fp32 [h*w][32]) and, if
+// given, cond16 (the fp16 operand of the fused SFT epilogues) of those rows.  AUTO reads K4_CONDNET_FP32 per call (fp32
+// FFMA kernel when it is "1").  num_cond 1 runs condnet_mma_kernel, a wider condition condnet_wide_mma_kernel.
 int run_condnet(const k4_srnet* n, const float* cond_in, int h, int w, int y_lo, int y_hi, float* cond32, __half* cond16,
                 cudaStream_t s, int sel = SRP_AUTO, int* used = nullptr) {
     bool fp32 = sel == SRP_FP32;
     if (sel == SRP_AUTO) { const char* cenv = getenv("K4_CONDNET_FP32"); fp32 = cenv && cenv[0] == '1'; }
+    const int nc = n->num_cond;
     if (fp32) {
-        CondParams cp{cond_in, n->condnet_w, cond32, h, w, y_lo, y_hi, cond16};
+        CondParams cp{cond_in, n->condnet_w, cond32, h, w, y_lo, y_hi, cond16, nc};
         constexpr int NW = 64 * 9 + 64 + 2 * (64 * 64 + 64) + 32 * 64 + 32;
-        if (int st = sr_set_smem(condnet_kernel, 11, NW * 4)) return st;
         const long long np = (long long)(y_hi - y_lo) * w;
-        K4_CUDA_TRY(sr_launch(condnet_kernel, (unsigned)((np + 127) / 128), 128, (size_t)NW * 4, s, cp));
+        if (nc == 1) {
+            if (int st = sr_set_smem(condnet_kernel<false>, 11, NW * 4)) return st;
+            K4_CUDA_TRY(sr_launch(condnet_kernel<false>, (unsigned)((np + 127) / 128), 128, (size_t)NW * 4, s, cp));
+        } else {
+            if (int st = sr_set_smem(condnet_kernel<true>, 13, NW * 4)) return st;
+            K4_CUDA_TRY(sr_launch(condnet_kernel<true>, (unsigned)((np + 127) / 128), 128, (size_t)NW * 4, s, cp));
+        }
+    } else if (nc > 1) {
+        const CondMmaParams cp{cond_in, n->condnet_mma, cond32, cond16, h, w, y_lo, y_hi, nc};
+        const int nks = (nc + 15) / 16;
+        const int st = nks == 1 ? launch_condnet_wide<1>(cp, s) : nks == 2 ? launch_condnet_wide<2>(cp, s)
+                     : nks == 3 ? launch_condnet_wide<3>(cp, s) : launch_condnet_wide<4>(cp, s);
+        if (st) return st;
     } else {
-        CondMmaParams cp{cond_in, n->condnet_mma, cond32, cond16, h, w, y_lo, y_hi};
+        CondMmaParams cp{cond_in, n->condnet_mma, cond32, cond16, h, w, y_lo, y_hi, nc};
         const int smem = cnm_layout().total;
         if (int st = sr_set_smem(condnet_mma_kernel, 12, smem)) return st;
         const long long nb = ((long long)(y_hi - y_lo) * w + 15) / 16;
@@ -1438,9 +1598,12 @@ extern "C" int k4_srnet_destroy(k4_srnet* n) {
 extern "C" int k4_srnet_create(const k4_srnet_desc* d, k4_stream_t stream, k4_srnet** out) {
     if (!d || !out || !d->h_params) return K4_ERR_INVALID_ARG;
     *out = nullptr;
-    if (d->num_feat != 64 || d->num_grow_ch != 32 || d->num_cond != 1 || d->n_in_colors != 3 || (d->scale != 4 && d->scale != 1) ||
+    if (d->num_cond < 1) return K4_ERR_INVALID_ARG;
+    // the shipped configurations (run_sr.py:1353; x1 as in the 1x configs) with a condition of up to 64 channels (depth,
+    // the view embedding, or both: run_sr.py:895-912); others are not built
+    if (d->num_feat != 64 || d->num_grow_ch != 32 || d->num_cond > 64 || d->n_in_colors != 3 || (d->scale != 4 && d->scale != 1) ||
         d->num_block < 1 || d->num_block > 32)
-        return K4_ERR_UNSUPPORTED;          // the shipped configurations (run_sr.py:1353; x1 as in the 1x configs); others are not built
+        return K4_ERR_UNSUPPORTED;
     const bool up = d->scale == 4;          // x1 registers no conv_up1 / conv_up2 (lib/sr_esrnet.py:430-433)
     const int expect = 2 * (1 + 4 + d->num_block * (3 * 13 + 4) + 4 + (up ? 5 : 3));
     if (d->n_params != expect) return K4_ERR_INVALID_ARG;
@@ -1451,12 +1614,12 @@ extern "C" int k4_srnet_create(const k4_srnet_desc* d, k4_stream_t stream, k4_sr
     k4_srnet* n = new (std::nothrow) k4_srnet();
     if (!n) return K4_ERR_INVALID_ARG;
     memset(n, 0, sizeof(*n));
-    n->num_feat = 64; n->num_block = d->num_block; n->num_grow = 32; n->num_cond = 1; n->n_in = 3; n->scale = d->scale;
+    n->num_feat = 64; n->num_block = d->num_block; n->num_grow = 32; n->num_cond = d->num_cond; n->n_in = 3; n->scale = d->scale;
     const float* const* P = d->h_params;
     int k = 0;
 #define SR_TRY(x) do { st = (x); if (st != K4_OK) { k4_srnet_destroy(n); return st; } } while (0)
     SR_TRY(make_conv(n, n->conv_first, P[k], P[k + 1], 64, 3, s)); k += 2;
-    SR_TRY(make_condnet(n, P + k, s)); k += 8;
+    SR_TRY(make_condnet(n, P + k, n->num_cond, s)); k += 8;
     for (int i = 0; i < d->num_block; ++i) {
         for (int j = 0; j < 3; ++j) {
             for (int c = 0; c < 5; ++c) {
@@ -1787,6 +1950,7 @@ extern "C" int k4_testing_condnet(const k4_condnet_test_args* a, int32_t* kernel
     if (a->H < 1 || a->W < 1 || (long long)a->H * a->W > (1LL << 30)) return K4_ERR_INVALID_ARG;
     if (a->y_lo < 0 || a->y_lo >= a->y_hi || a->y_hi > a->H) return K4_ERR_INVALID_ARG;
     if (a->kernel < SRP_AUTO || a->kernel > SRP_FP32) return K4_ERR_INVALID_ARG;
+    if (a->num_cond < 0 || a->num_cond > 64) return K4_ERR_INVALID_ARG;
     if (((uintptr_t)a->d_cond_in & 3) || ((uintptr_t)a->d_cond_out & 7) || ((uintptr_t)a->d_cond16 & 3)) return K4_ERR_INVALID_ARG;
     int st = k4_device_check();
     if (st != K4_OK) return st;
@@ -1795,8 +1959,9 @@ extern "C" int k4_testing_condnet(const k4_condnet_test_args* a, int32_t* kernel
     k4_srnet* n = new (std::nothrow) k4_srnet();
     if (!n) return K4_ERR_INVALID_ARG;
     memset(n, 0, sizeof(*n));
+    n->num_cond = a->num_cond ? a->num_cond : 1;
     int used = -1;
-    st = make_condnet(n, a->h_condnet, s);
+    st = make_condnet(n, a->h_condnet, n->num_cond, s);
     if (!st) st = run_condnet(n, a->d_cond_in, a->H, a->W, a->y_lo, a->y_hi, a->d_cond_out, static_cast<__half*>(a->d_cond16), s,
                               a->kernel, &used);
     const cudaError_t e = cudaStreamSynchronize(s);       // the packs are freed below

@@ -89,7 +89,7 @@ class CondnetTestArgs(C.Structure):
     _fields_ = [
         ('h_condnet', C.POINTER(C.c_void_p)), ('d_cond_in', C.c_void_p), ('H', C.c_int32), ('W', C.c_int32),
         ('y_lo', C.c_int32), ('y_hi', C.c_int32), ('d_cond_out', C.c_void_p), ('d_cond16', C.c_void_p),
-        ('kernel', C.c_int32), ('reserved0', C.c_int32),
+        ('kernel', C.c_int32), ('num_cond', C.c_int32),
     ]
 
 

@@ -444,9 +444,10 @@ def sr_plan(H, W, tile_size, tile_pad, world, halo):
 
 def sr_decode_sharded(net_fn, img, cond, tile_size, tile_pad=10, scale=4, halo=80, group=None, net_units_fn=None,
                       peers=None):
-    """x`scale` decode of ``img [1,C,H,W]`` / ``cond [1,H,W]`` (full frame on every rank) with the units
+    """x`scale` decode of ``img [1,C,H,W]`` / ``cond [num_cond,H,W]`` (full frame on every rank; ``num_cond`` 1 for the
+    depth condition, 63 / 64 for the view-conditioned decoder) with the units
     of :func:`sr_units` dealt round-robin over the ranks and ONE all-gather of the packed output
-    blocks.  ``net_fn(img_crop, cond_crop[1,1,h,w]) -> [1,C,scale*h,scale*w]`` is the decoder
+    blocks.  ``net_fn(img_crop, cond_crop[1,num_cond,h,w]) -> [1,C,scale*h,scale*w]`` is the decoder
     (``SFTNet.forward``); ``net_units_fn(jobs)`` with ``jobs = [(img_crop, cond_crop, (y0,y1,x0,x1), out[C,.,.]), ...]``
     (``SFTNet.run_units``), when given, writes every unit's kept block straight into the packed send buffer, lets every
     layer skip the rows outside the kept block's remaining receptive field and overlaps a rank's units on two

@@ -164,8 +164,12 @@ def render_frame_4k(model, net_sr, H, W, K, c2w, ndc, render_kwargs, test_tile=5
     1x configs) with the reference's tile geometry (``--test_tile``), optional ``to8b`` quantisation (lib/utils.py:20)
     on the device.
 
+    The decoder's condition is :func:`k4nerf.sr_esrnet.sft_condition` of ``net_sr.num_cond``: the depth, the view
+    embedding of the frame's ``viewdirs``, or both.
+
     Returns ``(sr [3,s*H,s*W] float32 in [0,1] or uint8 [s*H,s*W,3], lr dict)`` -- same values as
     ``render_viewpoints_sr`` followed by ``SFTNet.tile_process`` and ``clamp(0,1)``."""
+    from .sr_esrnet import sft_condition
     rays_o, rays_d, viewdirs = dvgo.get_rays_of_a_view(
         H, W, K, torch.as_tensor(np.asarray(c2w), dtype=torch.float32), ndc,
         inverse_y=render_kwargs['inverse_y'], flip_x=flip_x, flip_y=flip_y)
@@ -173,7 +177,7 @@ def render_frame_4k(model, net_sr, H, W, K, c2w, ndc, render_kwargs, test_tile=5
     kw['render_depth'] = True
     lr = model.render_rays(rays_o.view(-1, 3), rays_d.view(-1, 3), viewdirs.view(-1, 3), kw, image_hw=(H, W))
     x = lr['rgb_marched'].view(H, W, 3).permute(2, 0, 1).unsqueeze(0).contiguous()    # unclamped, as run_sr.py:131
-    cond = lr['depth'].view(1, H, W)
+    cond = sft_condition(net_sr.num_cond, lr['depth'], viewdirs, H, W)
     sr = net_sr.tile_process(x, cond, tile_size=test_tile if test_tile else max(H, W), to_cpu=False)
     sr = sr.squeeze(0).clamp_(0, 1)
     if out_u8:
@@ -190,8 +194,10 @@ def render_frame_4k_sharded(model, net_sr, H, W, K, c2w, ndc, render_kwargs, tes
     reference tiles / tile row-parts (one all-gather of the decoded blocks, x``net_sr.scale``).  Every rank returns the
     full frame; values are identical to the single-GPU :func:`render_frame_4k`.  The LR dict's tensors are views of the
     cached :class:`k4nerf.dist.CyclicFrame` buffer (no allocation per frame): valid until the next call with the same
-    (H, W, group)."""
+    (H, W, group).  A view-conditioned decoder (``net_sr.num_cond`` 63 / 64) needs the whole frame's ``viewdirs``: every
+    rank generates them itself (they depend on ``K`` and ``c2w`` only), so nothing more is exchanged."""
     from . import dist as kdist
+    from .sr_esrnet import sft_condition
     kw = dict(render_kwargs)
     kw['render_depth'] = True
     dev = next(model.parameters()).device
@@ -206,7 +212,11 @@ def render_frame_4k_sharded(model, net_sr, H, W, K, c2w, ndc, render_kwargs, tes
     fn = lambda ro, rd, vd, hw, out: model.render_rays(ro, rd, vd, kw, image_hw=hw, out=out)
     lr = frame.render(make, fn)          # rank's rays only -> fused march into the packed buffer -> one all-gather -> transpose
     x = lr['rgb_marched'].view(H, W, 3).permute(2, 0, 1).unsqueeze(0).contiguous()
-    cond = lr['depth'].view(1, H, W).contiguous()
+    viewdirs = None
+    if net_sr.num_cond != 1:
+        viewdirs = dvgo.get_rays_of_a_view(H, W, K, c2w_t, ndc, inverse_y=render_kwargs['inverse_y'], flip_x=flip_x,
+                                           flip_y=flip_y, device=dev)[2]
+    cond = sft_condition(net_sr.num_cond, lr['depth'], viewdirs, H, W).contiguous()
     sr = net_sr.tile_process_sharded(x, cond, tile_size=test_tile if test_tile else max(H, W), group=group)
     sr = sr.squeeze(0).clamp_(0, 1)
     if out_u8:

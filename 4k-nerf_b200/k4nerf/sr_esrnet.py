@@ -52,6 +52,36 @@ class RRDB_SFT(nn.Module):
         self.sft0 = SFTLayer(num_feat, num_grow_ch)
 
 
+def sft_condition(num_cond, depth, viewdirs, H, W):
+    """The SFT condition ``[num_cond, H, W]`` of an H x W LR frame, the one run_sr.py selects with
+    ``cfg.fine_model_and_render.num_cond`` before every decoder call:
+
+    * 1: the marched depth (run_sr.py:895-898, :1365-1367);
+    * 63: the view-direction embedding at every pixel, ``[v, sin(v * 2^i), cos(v * 2^i)]``, i = 0..9, v = the pixel's
+      normalised ``viewdirs``; the 30 sin (cos) channels ordered by direction axis first, frequency second
+      (run_sr.py:899-904, :1368-1373);
+    * 64: depth as channel 0, then the 63 channels above -- the training path's ``torch.cat((depth, emb), 1)``
+      (run_sr.py:905-912).  The reference's validation, test and video paths fail for 64 (they index a 3-D depth with
+      four indices, run_sr.py:1376, or concatenate 3-D with 4-D tensors), so the training path defines it.
+
+    ``depth``: ``H*W`` values (any shape of that size), ``viewdirs``: ``[H*W, 3]`` (or ``[H, W, 3]``), on one device.
+    The embedding uses run_sr.py's own torch expressions, so on the same device its values equal the reference's bit for
+    bit.  Other ``num_cond`` values raise: the reference's driver defines no other condition."""
+    H, W = int(H), int(W)
+    if num_cond not in (1, 63, 64):
+        raise ValueError(f'run_sr.py defines the SFT condition for num_cond 1, 63 and 64 only, got {num_cond!r}')
+    if num_cond == 1:
+        return depth.reshape(1, H, W)
+    viewdirs = viewdirs.reshape(H * W, 3)
+    viewfreq = torch.FloatTensor([(2**i) for i in range(10)]).to(viewdirs.device)
+    emb = (viewdirs.unsqueeze(-1) * viewfreq).flatten(-2)
+    emb = torch.cat([viewdirs, emb.sin(), emb.cos()], -1)
+    emb = emb.reshape(H, W, -1).movedim(-1, 0)
+    if num_cond == 63:
+        return emb.contiguous()
+    return torch.cat((depth.reshape(1, H, W).to(emb.dtype), emb), 0)
+
+
 class _NetHandle:
     def __init__(self, ptr, fingerprint):
         self.ptr, self.fingerprint = ptr, fingerprint
@@ -68,10 +98,14 @@ class _NetHandle:
 class SFTNet(nn.Module):
     def __init__(self, n_in_colors, scale, num_feat=64, num_block=5, num_grow_ch=32, num_cond=1, dswise=False):
         super().__init__()
-        if dswise or n_in_colors != 3 or scale not in (1, 4) or num_feat != 64 or num_grow_ch != 32 or num_cond != 1:
-            raise NotImplementedError('k4nerf builds the shipped VC-Decoders: SFTNet(3, 4, 64, n, 32, 1) (run_sr.py:1353) and '
-                                      'SFTNet(3, 1, 64, n, 32, 1) (the 1x configs)')
+        if int(num_cond) != num_cond or num_cond < 1:
+            raise ValueError(f'num_cond must be a positive integer (the condition channels of CondNet.0), got {num_cond!r}')
+        num_cond = int(num_cond)
+        if dswise or n_in_colors != 3 or scale not in (1, 4) or num_feat != 64 or num_grow_ch != 32 or num_cond > 64:
+            raise NotImplementedError('k4nerf builds the shipped VC-Decoders: SFTNet(3, 4, 64, n, 32, c) (run_sr.py:1353) and '
+                                      'SFTNet(3, 1, 64, n, 32, c) (the 1x configs) with a condition of c = 1..64 channels')
         self.scale = scale
+        self.num_cond = num_cond
         self.dswise = dswise
         self.conv_first = nn.Conv2d(n_in_colors, num_feat, 3, 1, 1)
         self.body = nn.Sequential(*[RRDB_SFT(num_feat=num_feat, num_grow_ch=num_grow_ch) for _ in range(num_block)])
@@ -136,14 +170,14 @@ class SFTNet(nn.Module):
     @torch.no_grad()
     def forward_roi(self, x, cond, keep, out, ws_slot=0, extra=None):
         """The output pixels (``s = self.scale`` per LR pixel and axis) of LR block ``keep = (y0, y1, x0, x1)`` of tile
-        ``x [1,3,h,w]`` / ``cond [1,1,h,w]`` written into ``out``: a ``[3, s(y1-y0), s(x1-x0)]`` fp32 CUDA view with unit
+        ``x [1,3,h,w]`` / ``cond [1,num_cond,h,w]`` written into ``out``: a ``[3, s(y1-y0), s(x1-x0)]`` fp32 CUDA view with unit
         stride along x (typically a window of the frame).  Same values as ``forward(x, cond)[0, :, s*y0:s*y1, s*x0:s*x1]``;
         every layer computes only the rows inside the
         remaining receptive field of the kept rows (k4_srnet_forward_roi).  Runs on the current stream.  ``extra``: device
         pointers (ints) of the same window in other ranks' peer-mapped frames -- the last convolution stores the block there
         too (k4_srnet_forward_roi_peers)."""
         require_cuda(x, cond, out)
-        assert x.dim() == 4 and x.shape[0] == 1 and x.shape[1] == 3 and cond.shape[1] == 1, 'batch 1, 3+1 channels'
+        self._check_inputs(x, cond)
         h, w = int(x.shape[2]), int(x.shape[3])
         y0, y1, x0, x1 = [int(v) for v in keep]
         s = self.scale
@@ -170,11 +204,14 @@ class SFTNet(nn.Module):
 
     @torch.no_grad()
     def run_units(self, jobs, streams=2):
-        """``forward_roi`` for a list of independent jobs ``(x_crop, cond_crop, keep, out_view[, extra])`` dealt (largest first) to
+        """``forward_roi`` for a list of independent jobs ``(x_crop [1,3,h,w], cond_crop [1,num_cond,h,w], keep, out_view[, extra])``
+        dealt (largest first) to
         ``streams`` CUDA streams with a workspace each; returns when the current stream has been made to wait for all of
         them.  Independent units overlap each other's launch / fill / drain phases (~120 kernels per unit)."""
         if not jobs:
             return
+        for job in jobs:
+            self._check_inputs(job[0], job[1])
         dev = jobs[0][0].device
         n_streams = max(1, min(int(streams), len(jobs)))
         cur = torch.cuda.current_stream(dev)
@@ -207,11 +244,11 @@ class SFTNet(nn.Module):
 
     @torch.no_grad()
     def forward(self, x, cond, fea=None):
-        """x [1,3,h,w], cond [1,1,h,w] (CUDA, fp32) -> [1,3,s*h,s*w], s = self.scale  (lib/sr_esrnet.py:446-465)."""
+        """x [1,3,h,w], cond [1,num_cond,h,w] (CUDA, fp32) -> [1,3,s*h,s*w], s = self.scale  (lib/sr_esrnet.py:446-465)."""
         if fea is not None:
             raise NotImplementedError('the `fea` branch needs conv_prefea (n_in_colors > 3), not in the shipped config')
         require_cuda(x, cond)
-        assert x.dim() == 4 and x.shape[0] == 1 and x.shape[1] == 3 and cond.shape[1] == 1, 'batch 1, 3+1 channels'
+        self._check_inputs(x, cond)
         h, w = int(x.shape[2]), int(x.shape[3])
         out = torch.empty((1, 3, h * self.scale, w * self.scale), device=x.device, dtype=torch.float32)
         self.forward_roi(x, cond, (0, h, 0, w), out[0])
@@ -224,9 +261,13 @@ class SFTNet(nn.Module):
         written by the last convolution straight into the frame (no crop copies), the frame is assembled on
         the device and moved to the CPU once (the reference copies every tile), and the tiles are dealt to
         ``streams`` CUDA streams with a workspace each: the tiles are independent, so the launch / fill /
-        drain phases of one tile's ~120 kernels overlap the other tile's work."""
+        drain phases of one tile's ~120 kernels overlap the other tile's work.
+
+        ``img [1,3,H,W]``, ``cond [num_cond,H,W]``: the condition is unsqueezed inside, as the reference does (:474).  A 4-D
+        condition raises (the reference would slice the wrong axes of it)."""
         batch, channel, height, width = img.shape
         assert batch == 1
+        self._check_frame_cond(cond, height, width)
         cond = cond.unsqueeze(0)
         s = self.scale
         dev = img.device
@@ -246,6 +287,19 @@ class SFTNet(nn.Module):
         self.run_units(jobs, streams)
         return output.to('cpu') if to_cpu else output
 
+    def _check_inputs(self, x, cond):
+        """A tile: x [1,3,h,w] and cond [1,num_cond,h,w]."""
+        assert x.dim() == 4 and x.shape[0] == 1 and x.shape[1] == 3, f'x must be [1,3,h,w], got {tuple(x.shape)}'
+        if cond.dim() != 4 or cond.shape[0] != 1 or cond.shape[1] != self.num_cond or cond.shape[2:] != x.shape[2:]:
+            raise ValueError(f'cond must be [1,{self.num_cond},{x.shape[2]},{x.shape[3]}] (num_cond = {self.num_cond}), '
+                             f'got {tuple(cond.shape)}')
+
+    def _check_frame_cond(self, cond, height, width):
+        """A frame's condition for tile_process: [num_cond,H,W], the reference's contract (lib/sr_esrnet.py:474)."""
+        if cond.dim() != 3 or tuple(cond.shape) != (self.num_cond, height, width):
+            raise ValueError(f'tile_process takes cond [num_cond,H,W] = [{self.num_cond},{height},{width}] and unsqueezes it '
+                             f'itself (lib/sr_esrnet.py:474), got {tuple(cond.shape)}')
+
     def receptive_halo(self):
         """LR rows a decoded pixel can depend on above/below it: conv_first/CondNet.0 (1) + 15 3x3 convs
         per RRDB_SFT + conv_body (1) + the tail, rounded up to an even count.  The tail is the 3x3 convs behind
@@ -263,9 +317,10 @@ class SFTNet(nn.Module):
         full frame as single-GPU ``tile_process`` (device resident).  On the GPUs of one node every unit's last
         convolution stores its kept block straight into every rank's frame (peer-mapped, :class:`k4nerf.dist.PeerBuffers`;
         two frames alternate, the returned one is valid until the call after the next one); otherwise one all-gather of
-        the packed blocks + assembly."""
+        the packed blocks + assembly.  ``cond [num_cond,H,W]`` as in :meth:`tile_process`."""
         from . import dist as kdist
         batch, channel, height, width = img.shape
+        self._check_frame_cond(cond, height, width)
         peers = None
         if img.is_cuda and kdist.dist.is_initialized():
             cache = self.__dict__.setdefault('_k4_peer_frames', {})

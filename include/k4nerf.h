@@ -230,8 +230,10 @@ K4_API int k4_make_rays_rows(const float* h_K, const float* h_c2w, int32_t H, in
  *     scale 1: conv_body; conv_hr; conv_last.
  * n_params = 2 * (1 + 4 + 43 * num_block + 4 + (scale == 4 ? 5 : 3)): 229 convolutions for 5 blocks at x4, 227 at x1;
  * a count that does not match the scale returns K4_ERR_INVALID_ARG.
- * Only SFTNet(n_in_colors=3, scale=4 or 1, num_feat=64, num_block<=32, num_grow_ch=32, num_cond=1, dswise=False)
- * (run_sr.py:1353) is built; other configurations, scale 2 included, return K4_ERR_UNSUPPORTED.
+ * Only SFTNet(n_in_colors=3, scale=4 or 1, num_feat=64, num_block<=32, num_grow_ch=32, num_cond=1..64, dswise=False)
+ * (run_sr.py:1353) is built; other configurations, scale 2 and num_cond > 64 included, return K4_ERR_UNSUPPORTED, and
+ * num_cond < 1 returns K4_ERR_INVALID_ARG.  num_cond is CondNet.0's input width (weight [64][num_cond][3][3]): 1 for the
+ * depth condition, 63 for the view-direction embedding, 64 for depth followed by the embedding (run_sr.py:895-912).
  */
 typedef struct k4_srnet_desc {
     int32_t n_in_colors, scale, num_feat, num_block, num_grow_ch, num_cond;
@@ -247,8 +249,8 @@ K4_API int k4_srnet_destroy(k4_srnet* net);
 K4_API size_t k4_srnet_workspace_bytes(const k4_srnet* net, int32_t h, int32_t w);
 
 /* Replaces: SFTNet.forward(x, cond) (lib/sr_esrnet.py:446-465) for one tile.
- * d_x [3,h,w], d_cond [1,h,w] planar fp32 (the reference's NCHW, batch 1); d_out [3,s*h,s*w] fp32 with s the net's
- * scale (4 or 1).
+ * d_x [3,h,w], d_cond [num_cond,h,w] planar fp32 (the reference's NCHW, batch 1); d_out [3,s*h,s*w] fp32 with s the
+ * net's scale (4 or 1).  The same d_cond layout holds for k4_srnet_forward_roi and k4_srnet_forward_roi_peers.
  * Tiling (SFTNet.tile_process, lib/sr_esrnet.py:467-527) is host logic above this call. */
 K4_API int k4_srnet_forward(const k4_srnet* net, const float* d_x, const float* d_cond, int32_t h, int32_t w,
                             float* d_out, void* d_workspace, size_t workspace_bytes, k4_stream_t stream);
@@ -434,11 +436,13 @@ K4_API int k4_testing_conv3x3(const k4_conv_test_args* args, int32_t* kernel_use
  *   sft_kernel, which run every valid shape.  *kernel_used (may be NULL) receives the kernel that ran, -1 on error.
  *   Arguments are checked before any CUDA call (K4_ERR_INVALID_ARG).  The calls synchronise `stream`.
  *
- * k4_testing_condnet: CondNet (conv3x3 1 -> 64, LeakyReLU 0.2, 1x1 64 -> 64, LeakyReLU, 1x1 64 -> 64, LeakyReLU,
+ * k4_testing_condnet: CondNet (conv3x3 num_cond -> 64, LeakyReLU 0.2, 1x1 64 -> 64, LeakyReLU, 1x1 64 -> 64, LeakyReLU,
  * 1x1 64 -> 32) on rows [y_lo, y_hi) of an H x W condition map, zero padded at the map's border.
- *   h_condnet: HOST array of the 8 device pointers in k4_srnet_desc order (CondNet.0 w [64][1][3][3], b [64], .2 w
- *   [64][64], b, .4 w [64][64], b, .6 w [32][64], b [32]).  d_cond_in fp32 [H][W].  d_cond_out fp32 [H*W][32] and d_cond16
- *   (fp16 [H*W][32], the operand of the fused SFT epilogues, NULL to skip) receive the window's rows only.
+ *   num_cond: 0 .. 64, 0 meaning 1 (other values: K4_ERR_INVALID_ARG).  MMA is condnet_mma_kernel at num_cond 1 and
+ *   condnet_wide_mma_kernel above.
+ *   h_condnet: HOST array of the 8 device pointers in k4_srnet_desc order (CondNet.0 w [64][num_cond][3][3], b [64], .2 w
+ *   [64][64], b, .4 w [64][64], b, .6 w [32][64], b [32]).  d_cond_in fp32 [num_cond][H][W].  d_cond_out fp32 [H*W][32]
+ *   and d_cond16 (fp16 [H*W][32], the operand of the fused SFT epilogues, NULL to skip) receive the window's rows only.
  *
  * k4_testing_sft: one SFT layer, y = x * (scale + 1) + shift, on pixels [p0, p0 + P) of per-pixel buffers.
  *   h_sft: HOST array of the layer's 8 device pointers (the h_sft convention of k4_conv_test_args); cout 32 or 64.
@@ -459,7 +463,7 @@ typedef struct k4_condnet_test_args {
     float* d_cond_out;
     void* d_cond16;                        /* fp16, or NULL */
     int32_t kernel;
-    int32_t reserved0;
+    int32_t num_cond;                      /* condition channels, 0 .. 64 (0: 1) */
 } k4_condnet_test_args;
 K4_API int k4_testing_condnet(const k4_condnet_test_args* args, int32_t* kernel_used, k4_stream_t stream);
 
