@@ -252,6 +252,11 @@ extern "C" int k4_scene_create(const k4_scene_desc* d, k4_stream_t stream, k4_sc
     if (d->rgbnet_depth < 0 || d->rgbnet_depth > K4_MAX_MLP_LAYERS || d->rgbnet_depth == 1) return K4_ERR_INVALID_ARG;
     if (d->kind == K4_KIND_DMPIGO && (!d->d_act_shift_grid || d->mpi_depth < 2)) return K4_ERR_INVALID_ARG;
     if (d->viewbase_pe < 0 || d->viewbase_pe > 10 || d->spatial_pe < 0 || d->spatial_pe > 10) return K4_ERR_UNSUPPORTED;
+    // the rgbnet's hidden activation: gauss / lkrelu exist in DirectMPIGO only (lib/dmpigo.py:89-95; DirectVoxGO and
+    // DirectContractedVoxGO hard-code ReLU), the Gaussian needs a finite a > 0
+    if (d->rgbnet_act != K4_ACT_RELU && d->rgbnet_act != K4_ACT_GAUSS && d->rgbnet_act != K4_ACT_LKRELU) return K4_ERR_INVALID_ARG;
+    if (d->rgbnet_act != K4_ACT_RELU && d->kind != K4_KIND_DMPIGO) return K4_ERR_INVALID_ARG;
+    if (d->rgbnet_act == K4_ACT_GAUSS && !(std::isfinite(d->rgbnet_act_param) && d->rgbnet_act_param > 0.f)) return K4_ERR_INVALID_ARG;
     const long long nvox = (long long)d->world_size[0] * d->world_size[1] * d->world_size[2];
     if (nvox >= (1ll << 31)) return K4_ERR_UNSUPPORTED;       // 32-bit voxel indices in the kernels
     int st = k4_device_check();
@@ -287,6 +292,13 @@ extern "C" int k4_scene_create(const k4_scene_desc* d, k4_stream_t stream, k4_sc
     for (int a = 0; a < 3; ++a) { v.scene_center[a] = d->scene_center[a]; v.scene_radius[a] = d->scene_radius[a]; }
     v.bg_len = d->bg_len; v.one_plus_bg = (float)(1.0 + (double)d->bg_len); v.world_len = d->world_len;
     if (d->kind == K4_KIND_DCVGO) v.direct = 1;
+    sc->act = d->rgbnet_depth > 0 ? d->rgbnet_act : K4_ACT_RELU;
+    if (sc->act == K4_ACT_GAUSS) {
+        const float a = d->rgbnet_act_param;
+        const float aa = a * a;
+        v.act_den = 2.f * aa;                                                  // torch: 2*self.a**2, in fp32
+        v.act_c = (float)(-1.4426950408889634 / (2.0 * (double)a * (double)a));  // -log2(e) / (2 a^2)
+    }
 
 #define K4_TRY(x) do { st = (x); if (st != K4_OK) { k4_scene_destroy(sc); return st; } } while (0)
 #define K4_CTRY(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { k4_set_cuda_error(_e, #x); k4_scene_destroy(sc); return K4_ERR_CUDA; } } while (0)
@@ -549,13 +561,13 @@ namespace {
 
 // F16 / F16X3: one warp per group of 32 rows, driven through MmaWarpCtx as k4_march_kernel drives it: push_row of the
 // group's rows (a full group flushes there), end_tile (flushes a partial group, hands back the per-lane accumulators).
-template <int MODE>
+template <int MODE, int ACT>
 __global__ void __launch_bounds__(K4_MARCH_THREADS)
 k4_test_rgbnet_mma_kernel(const __grid_constant__ K4Dev s, const float* __restrict__ xs, const float* __restrict__ diffs,
                           const float* __restrict__ ws, const int* __restrict__ owners, long long n, float* __restrict__ racc) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    MmaWarpCtx<MODE> mma;
+    MmaWarpCtx<MODE, ACT> mma;
     mma.init(s, smem_raw, warp, lane);
     const long long n_groups = (n + 31) / 32;
     for (long long g = (long long)blockIdx.x * K4_MARCH_WARPS + warp; g < n_groups; g += (long long)gridDim.x * K4_MARCH_WARPS) {
@@ -578,6 +590,7 @@ k4_test_rgbnet_mma_kernel(const __grid_constant__ K4Dev s, const float* __restri
 
 // FP32: thread (group g, owner j) walks the group's rows in order and accumulates the ones it owns, as k4_march_kernel
 // accumulates a ray's samples
+template <int ACT>
 __global__ void k4_test_rgbnet_fp32_kernel(const __grid_constant__ K4Dev s, const float* __restrict__ xs, const float* __restrict__ diffs,
                                            const float* __restrict__ ws, const int* __restrict__ owners, long long n,
                                            float* __restrict__ racc) {
@@ -589,7 +602,7 @@ __global__ void k4_test_rgbnet_fp32_kernel(const __grid_constant__ K4Dev s, cons
     for (long long r = g * 32; r < n && r < g * 32 + 32; ++r) {
         if ((owners[r] & 31) != j) continue;
         float rgb[3];
-        mlp_fp32(s, xs + r * s.dim0, rgb);
+        mlp_fp32<ACT>(s, xs + r * s.dim0, rgb);
         if (diffs) {
             rgb[0] = __fadd_rn(rgb[0], diffs[3 * r]); rgb[1] = __fadd_rn(rgb[1], diffs[3 * r + 1]);
             rgb[2] = __fadd_rn(rgb[2], diffs[3 * r + 2]);
@@ -603,9 +616,9 @@ __global__ void k4_test_rgbnet_fp32_kernel(const __grid_constant__ K4Dev s, cons
     racc[3 * i + 0] = acc_r; racc[3 * i + 1] = acc_g; racc[3 * i + 2] = acc_b;
 }
 
-template <int MODE>
+template <int MODE, int ACT>
 int launch_test_rgbnet_mma(const K4Dev& v, const k4_rgbnet_test_args* a, cudaStream_t st) {
-    auto kern = k4_test_rgbnet_mma_kernel<MODE>;
+    auto kern = k4_test_rgbnet_mma_kernel<MODE, ACT>;
     const size_t smem = MmaWarpCtx<MODE>::smem_bytes(v);
     if (smem > 48 * 1024) K4_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const long long n_groups = (a->n + 31) / 32;
@@ -616,13 +629,14 @@ int launch_test_rgbnet_mma(const K4Dev& v, const k4_rgbnet_test_args* a, cudaStr
     return K4_OK;
 }
 
+template <int ACT>
 int testing_rgbnet_mma(const K4Dev& v, const k4_rgbnet_test_args* a, cudaStream_t st) {
-    if (a->mode == K4_MLP_F16) return launch_test_rgbnet_mma<K4_MLP_F16>(v, a, st);
-    if (a->mode == K4_MLP_F16X3) return launch_test_rgbnet_mma<K4_MLP_F16X3>(v, a, st);
+    if (a->mode == K4_MLP_F16) return launch_test_rgbnet_mma<K4_MLP_F16, ACT>(v, a, st);
+    if (a->mode == K4_MLP_F16X3) return launch_test_rgbnet_mma<K4_MLP_F16X3, ACT>(v, a, st);
     if (a->mode != K4_MLP_FP32) return K4_ERR_UNSUPPORTED;
     const long long threads = (a->n + 31) / 32 * 32;
-    k4_test_rgbnet_fp32_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, st>>>(v, a->d_x, a->d_diffuse, a->d_w, a->d_owner, a->n,
-                                                                                 a->d_racc);
+    k4_test_rgbnet_fp32_kernel<ACT><<<(unsigned)((threads + 127) / 128), 128, 0, st>>>(v, a->d_x, a->d_diffuse, a->d_w, a->d_owner,
+                                                                                      a->n, a->d_racc);
     K4_CUDA_TRY(cudaGetLastError());
     return K4_OK;
 }
@@ -644,7 +658,10 @@ extern "C" int k4_testing_rgbnet(const k4_scene* sc, const k4_rgbnet_test_args* 
     if (a->mode == K4_MLP_F16 && !MmaWarpCtx<K4_MLP_F16>::supported(v)) return K4_ERR_UNSUPPORTED;
     if (a->mode == K4_MLP_F16X3 && !MmaWarpCtx<K4_MLP_F16X3>::supported(v)) return K4_ERR_UNSUPPORTED;
     cudaStream_t s = (cudaStream_t)stream;
-    int st = wgmma ? k4_testing_rgbnet_ws(sc, a, s) : testing_rgbnet_mma(v, a, s);
+    int st = wgmma ? k4_testing_rgbnet_ws(sc, a, s)
+           : sc->act == K4_ACT_GAUSS ? testing_rgbnet_mma<K4_ACT_GAUSS>(v, a, s)
+           : sc->act == K4_ACT_LKRELU ? testing_rgbnet_mma<K4_ACT_LKRELU>(v, a, s)
+                                      : testing_rgbnet_mma<K4_ACT_RELU>(v, a, s);
     const cudaError_t e = cudaStreamSynchronize(s);
     if (st == K4_OK && e != cudaSuccess) { k4_set_cuda_error(e, "k4_testing_rgbnet"); st = K4_ERR_CUDA; }
     if (st == K4_OK && group_rows) *group_rows = wgmma ? 128 : 32;

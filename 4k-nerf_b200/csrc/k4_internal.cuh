@@ -24,6 +24,10 @@ struct K4Dev {
     int dim0;                     // MLP input width (0 when depth == 0)
     int k0_view_off;              // first k0 channel fed to the MLP (3 when !direct, else 0)
     int n_in[K4_MAX_MLP_LAYERS], n_out[K4_MAX_MLP_LAYERS], ldw[K4_MAX_MLP_LAYERS];
+    // K4_ACT_GAUSS, fp32 mode: 2*(a*a) in fp32, the denominator of torch's -x**2/(2*a**2).  This field and act_c below
+    // sit in what was alignment padding, so no other field moves and the kernels without the activation keep their
+    // parameter layout.  The activation itself is a template parameter of the kernels (k4_scene::act selects them).
+    float act_den;
     const float* density;         // [X,Y,Z]
     const float* k0cl;            // [X,Y,Z,Cpad] channel last
     const uint8_t* mask;          // [mX,mY,mZ]
@@ -47,7 +51,8 @@ struct K4Dev {
     // DirectContractedVoxGO (lib/dcvgo.py)
     float scene_center[3], scene_radius[3], bg_len, one_plus_bg;
     int world_len;
-    const int* tc_colmap;         // [dim0]: column of every model input in the tc_cfg entry's row layout (k4_testing_rgbnet)
+    float act_c;                  // K4_ACT_GAUSS, tensor-core modes: -log2(e) / (2 a^2), from double (see act_den)
+    const int* tc_colmap;        // [dim0]: column of every model input in the tc_cfg entry's row layout (k4_testing_rgbnet)
 };
 
 // ---- wgmma operand blob (built by k4_scene_create, staged by one TMA bulk copy) -------------------
@@ -83,7 +88,9 @@ struct k4_scene {
     size_t bytes;
     void* allocs[64];
     int n_allocs;
+    int act;                      // K4_ACT_* of the rgbnet's hidden layers: which kernel instantiations run the scene
 };
+static_assert(sizeof(K4Dev) == 704, "K4Dev grew: the kernels' parameter layout would move");
 
 struct K4RenderParams {
     float near_, far_, stepdist, interval, bg, inv_nsamples;

@@ -77,16 +77,17 @@ __device__ __forceinline__ long long tile_ray(const K4RenderParams& rp, long lon
 }
 
 // ---------------------------------------------------------------------------------------------
-// The fused kernel.  KIND: K4_KIND_DVGO / K4_KIND_DMPIGO.  MODE: K4_MLP_FP32 or a tensor-core mode.
+// The fused kernel.  KIND: K4_KIND_DVGO / K4_KIND_DMPIGO.  MODE: K4_MLP_FP32 or a tensor-core mode.  ACT: the rgbnet's
+// hidden activation (K4_ACT_*); only DirectMPIGO is instantiated with the non-relu ones.
 // ---------------------------------------------------------------------------------------------
-template <int KIND, int MODE>
+template <int KIND, int MODE, int ACT>
 __global__ void __launch_bounds__(K4_MARCH_THREADS)
 k4_march_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4RenderParams rp) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
 
-    MmaWarpCtx<MODE> mma;
+    MmaWarpCtx<MODE, ACT> mma;
     if (MODE != K4_MLP_FP32) mma.init(s, smem_raw, warp, lane);
 
     unsigned long long tot_m = 0, tot_d = 0, tot_c = 0;
@@ -259,7 +260,7 @@ k4_march_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Rende
                             n += embed3(pe, s.spape, x + n);
                         }
                         for (int c = 0; c < n_vemb; ++c) x[n++] = vemb[c];
-                        mlp_fp32(s, x, rgb);
+                        mlp_fp32<ACT>(s, x, rgb);
                         if (KIND == K4_KIND_DVGO && !s.direct) {
                             rgb[0] = __fadd_rn(rgb[0], k0v[0]); rgb[1] = __fadd_rn(rgb[1], k0v[1]);
                             rgb[2] = __fadd_rn(rgb[2], k0v[2]);
@@ -305,9 +306,9 @@ k4_march_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Rende
     }
 }
 
-template <int KIND, int MODE>
+template <int KIND, int MODE, int ACT = K4_ACT_RELU>
 int launch_variant(const k4_scene* sc, const K4RenderParams& rp, cudaStream_t st) {
-    auto kern = k4_march_kernel<KIND, MODE>;
+    auto kern = k4_march_kernel<KIND, MODE, ACT>;
     size_t smem = MmaWarpCtx<MODE>::smem_bytes(sc->dev);
     if (smem > 48 * 1024) K4_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int dev = 0, sms = 0, per_sm = 0;
@@ -325,9 +326,24 @@ int launch_variant(const k4_scene* sc, const K4RenderParams& rp, cudaStream_t st
     return K4_OK;
 }
 
+// DirectMPIGO with a gauss / lkrelu rgbnet (act_type, lib/dmpigo.py:89-95)
+template <int ACT>
+int launch_mpi_act(const k4_scene* sc, const K4RenderParams& rp, int mlp_mode, cudaStream_t st) {
+    if (mlp_mode == K4_MLP_FP32 || sc->dev.depth == 0) return launch_variant<K4_KIND_DMPIGO, K4_MLP_FP32, ACT>(sc, rp, st);
+    if (mlp_mode == K4_MLP_F16 && MmaWarpCtx<K4_MLP_F16>::supported(sc->dev)) return launch_variant<K4_KIND_DMPIGO, K4_MLP_F16, ACT>(sc, rp, st);
+    if (mlp_mode == K4_MLP_F16X3 && MmaWarpCtx<K4_MLP_F16X3>::supported(sc->dev))
+        return launch_variant<K4_KIND_DMPIGO, K4_MLP_F16X3, ACT>(sc, rp, st);
+    return K4_ERR_UNSUPPORTED;
+}
+
 }  // namespace
 
 int k4_launch_march(const k4_scene* sc, const K4RenderParams& rp, int mlp_mode, cudaStream_t st) {
+    if (sc->act != K4_ACT_RELU) {           // k4_scene_create admits them for DirectMPIGO only
+        if (sc->dev.kind != K4_KIND_DMPIGO) return K4_ERR_UNSUPPORTED;
+        return sc->act == K4_ACT_GAUSS ? launch_mpi_act<K4_ACT_GAUSS>(sc, rp, mlp_mode, st)
+                                       : launch_mpi_act<K4_ACT_LKRELU>(sc, rp, mlp_mode, st);
+    }
     if (sc->dev.kind == K4_KIND_DCVGO) {
         if (mlp_mode == K4_MLP_FP32 || sc->dev.depth == 0) return launch_variant<K4_KIND_DCVGO, K4_MLP_FP32>(sc, rp, st);
         if (mlp_mode == K4_MLP_F16 && MmaWarpCtx<K4_MLP_F16>::supported(sc->dev)) return launch_variant<K4_KIND_DCVGO, K4_MLP_F16>(sc, rp, st);

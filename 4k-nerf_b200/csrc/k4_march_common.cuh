@@ -241,7 +241,41 @@ __device__ __forceinline__ int embed3(const float v[3], int nfreq, float* out) {
     return n;
 }
 
-// fp32 rgbnet: Linear-ReLU-...-Linear, sequential FMA from the bias (exact mode).
+// The rgbnet's hidden activation (K4_ACT_*, include/k4nerf.h), the one definition every MLP path uses.
+//   fp32(x)  the fp32 mode: torch's own expression order, so that mode stays the exact cross-check
+//            gauss:  -x**2 / (2*a**2) -> t = x*x; t = -t; expf(t / den) with den = 2*(a*a) rounded in fp32 on the host
+//            lkrelu: ATen leaky_relu, x > 0 ? x : x * negval
+//   tc(x)    the tensor-core modes, on the fp32 accumulator before the one rounding to fp16:
+//            gauss:  ex2.approx(x*x*c), c = -log2(e) / (2 a^2) (k4_scene_create); +-inf and huge x give exactly 0
+// relu is fmaxf(x, 0) in both (the wgmma repack fuses it into cvt.rn.relu, see mlp_act_h2 in k4_march_mlp.cuh).
+template <int ACT>
+struct RgbAct {
+    static_assert(ACT == K4_ACT_RELU || ACT == K4_ACT_GAUSS || ACT == K4_ACT_LKRELU, "K4_ACT_*");
+    __device__ __forceinline__ static float fp32(float x, const K4Dev& s) {
+        if constexpr (ACT == K4_ACT_GAUSS) {
+            const float t = -__fmul_rn(x, x);
+            return expf(__fdiv_rn(t, s.act_den));
+        } else if constexpr (ACT == K4_ACT_LKRELU) {
+            return x > 0.f ? x : __fmul_rn(x, 0.01f);
+        } else {
+            return fmaxf(x, 0.f);
+        }
+    }
+    __device__ __forceinline__ static float tc(float x, float c) {
+        if constexpr (ACT == K4_ACT_GAUSS) {
+            float y;
+            asm("ex2.approx.ftz.f32 %0, %1;\n" : "=f"(y) : "f"(__fmul_rn(__fmul_rn(x, x), c)));
+            return y;
+        } else if constexpr (ACT == K4_ACT_LKRELU) {
+            return x > 0.f ? x : __fmul_rn(x, 0.01f);
+        } else {
+            return fmaxf(x, 0.f);
+        }
+    }
+};
+
+// fp32 rgbnet: Linear-act-...-Linear, sequential FMA from the bias (exact mode).
+template <int ACT>
 __device__ __noinline__ void mlp_fp32(const K4Dev& s, const float* x, float rgb[3]) {
     float bufA[K4_MAX_WIDTH], bufB[K4_MAX_WIDTH];
     const float* in = x;
@@ -262,8 +296,8 @@ __device__ __noinline__ void mlp_fp32(const K4Dev& s, const float* x, float rgb[
             if (last) {
                 rgb[0] = acc.x; rgb[1] = acc.y; rgb[2] = acc.z;
             } else {
-                out[j + 0] = fmaxf(acc.x, 0.f); out[j + 1] = fmaxf(acc.y, 0.f);
-                out[j + 2] = fmaxf(acc.z, 0.f); out[j + 3] = fmaxf(acc.w, 0.f);
+                out[j + 0] = RgbAct<ACT>::fp32(acc.x, s); out[j + 1] = RgbAct<ACT>::fp32(acc.y, s);
+                out[j + 2] = RgbAct<ACT>::fp32(acc.z, s); out[j + 3] = RgbAct<ACT>::fp32(acc.w, s);
             }
         }
         in = out;

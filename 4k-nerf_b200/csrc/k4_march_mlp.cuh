@@ -2,7 +2,8 @@
 //
 // One warpgroup runs a batch of 128 queued sample rows through the three layers, 64 rows (one wgmma M) at a time:
 //   L1  acc[64 x W] = A(ring tile, smem) * W1(smem) + bias             wgmma SS, fp32 accumulate in registers
-//   E1  cvt.rn.relu.f16x2 of the accumulator = the A fragments of L2   (no trip through shared memory)
+//   E1  activation + cvt to fp16x2 of the accumulator = the A fragments of L2   (no trip through shared memory;
+//       relu is the fused cvt.rn.relu.f16x2, gauss / lkrelu are evaluated in fp32 first: mlp_act_h2)
 //   L2  acc[64 x W] = H1(registers) * W2(smem) + bias                  wgmma RS
 //   E2  same repack -> H2
 //   L3  acc[64 x 16] = H2(registers) * W3(smem) + bias -> sigmoid -> weight -> shared-memory atomicAdd into the ray
@@ -18,14 +19,28 @@ __device__ __forceinline__ uint32_t mlp_relu_h2(float lo, float hi) {
     return d;
 }
 
-// 64 accumulator columns (block nc of a hidden layer) -> ReLU'd fp16 A fragments of k16 steps 4*nc .. 4*nc+3
-__device__ __forceinline__ void mlp_repack(const float (&acc)[32], uint32_t (*h)[4]) {
+// act(lo), act(hi) as one fp16x2 word: relu stays the fused cvt.rn.relu; the other activations are evaluated in fp32
+// on the accumulator (RgbAct::tc, c = K4Dev::act_c) and rounded once.
+template <int ACT>
+__device__ __forceinline__ uint32_t mlp_act_h2(float lo, float hi, float c) {
+    if constexpr (ACT == K4_ACT_RELU) {
+        return mlp_relu_h2(lo, hi);
+    } else {
+        uint32_t d;
+        asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;\n" : "=r"(d) : "f"(RgbAct<ACT>::tc(hi, c)), "f"(RgbAct<ACT>::tc(lo, c)));
+        return d;
+    }
+}
+
+// 64 accumulator columns (block nc of a hidden layer) -> activated fp16 A fragments of k16 steps 4*nc .. 4*nc+3
+template <int ACT>
+__device__ __forceinline__ void mlp_repack(const float (&acc)[32], uint32_t (*h)[4], float c) {
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
-        h[q][0] = mlp_relu_h2(acc[8 * q + 0], acc[8 * q + 1]);     // row g,     k 2t, 2t+1
-        h[q][1] = mlp_relu_h2(acc[8 * q + 2], acc[8 * q + 3]);     // row g + 8
-        h[q][2] = mlp_relu_h2(acc[8 * q + 4], acc[8 * q + 5]);     // row g,     k 2t+8, 2t+9
-        h[q][3] = mlp_relu_h2(acc[8 * q + 6], acc[8 * q + 7]);     // row g + 8
+        h[q][0] = mlp_act_h2<ACT>(acc[8 * q + 0], acc[8 * q + 1], c);     // row g,     k 2t, 2t+1
+        h[q][1] = mlp_act_h2<ACT>(acc[8 * q + 2], acc[8 * q + 3], c);     // row g + 8
+        h[q][2] = mlp_act_h2<ACT>(acc[8 * q + 4], acc[8 * q + 5], c);     // row g,     k 2t+8, 2t+9
+        h[q][3] = mlp_act_h2<ACT>(acc[8 * q + 6], acc[8 * q + 7], c);     // row g + 8
     }
 }
 
@@ -110,11 +125,12 @@ __device__ __forceinline__ void mlp_epilogue(const MlpEpiRows& e, float* racc, i
 // already fill the ring, unless colour_first is set; then consumed() also means "colours accumulated".  Running the
 // first half's epilogue under the second half's L1 MMAs instead keeps the accumulator, the epilogue and its inputs
 // live at once: the 128-wide configurations then need 150 registers of the 128 and ptxas serialises the wgmmas (C7518).
-// `mark` receives the phase boundaries (PhaseClock).
-template <int W, int KPAD, bool DIRECT, class Consumed, class Mark = NoPhases>
+// `mark` receives the phase boundaries (PhaseClock).  ACT: the hidden activation of E1 / E2 (K4_ACT_*), act_c its
+// constant (K4Dev::act_c; unused by relu).
+template <int W, int KPAD, bool DIRECT, int ACT, class Consumed, class Mark = NoPhases>
 __device__ __forceinline__ void mlp_batch_wgmma(uint32_t a_tile, const unsigned char* blob, const TcBlobLayout& BL, int valid,
                                                 unsigned slot0, const float* qw, const unsigned char* qowner, const float* qdiff,
-                                                float* racc, int wt, const Consumed& consumed, bool colour_first,
+                                                float* racc, int wt, float act_c, const Consumed& consumed, bool colour_first,
                                                 const Mark& mark = Mark()) {
     constexpr int KCH = KPAD / 8, KCHW = W / 8, NC = W / 64;      // NC: 64-column blocks of a hidden layer
     static_assert(W % 64 == 0, "hidden width");
@@ -144,7 +160,7 @@ __device__ __forceinline__ void mlp_batch_wgmma(uint32_t a_tile, const unsigned 
             wg_fence_acc(acc);
             mark(K4_PH_L_L1);
 #pragma unroll
-            for (int nc = 0; nc < NC; ++nc) mlp_repack(*reinterpret_cast<const float (*)[32]>(acc + 32 * nc), h1 + 4 * nc);
+            for (int nc = 0; nc < NC; ++nc) mlp_repack<ACT>(*reinterpret_cast<const float (*)[32]>(acc + 32 * nc), h1 + 4 * nc, act_c);
             mark(K4_PH_L_REPACK);
         }
         {
@@ -158,7 +174,7 @@ __device__ __forceinline__ void mlp_batch_wgmma(uint32_t a_tile, const unsigned 
             wg_fence_acc(acc);
             mark(K4_PH_L_L2);
 #pragma unroll
-            for (int nc = 0; nc < NC; ++nc) mlp_repack(*reinterpret_cast<const float (*)[32]>(acc + 32 * nc), h2 + 4 * nc);
+            for (int nc = 0; nc < NC; ++nc) mlp_repack<ACT>(*reinterpret_cast<const float (*)[32]>(acc + 32 * nc), h2 + 4 * nc, act_c);
             mark(K4_PH_L_REPACK);
         }
         float o[8];

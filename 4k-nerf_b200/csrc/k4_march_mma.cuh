@@ -6,7 +6,7 @@
 // Each warp owns a 64-row ring of fp16 feature rows in shared memory.  Lanes whose sample survived
 // the alpha / weight thresholds append one row (ballot + popc slot assignment); whenever 32 rows
 // are pending the warp runs the whole MLP for them with mma.sync.m16n8k16 (fp16 operands, fp32
-// accumulate):  layer-1 accumulators are ReLU'd and re-packed IN REGISTERS as the A fragments of
+// accumulate):  layer-1 accumulators are activated and re-packed IN REGISTERS as the A fragments of
 // layer 2 (the C-fragment layout of two n8 tiles is exactly one k16 A fragment), layer-2 output is
 // consumed 16 columns at a time by layer 3, so no activation ever touches shared memory.  Weights
 // ([n][k] fp16, k contiguous, +16 B row padding => conflict-free ldmatrix) are staged once per CTA
@@ -107,7 +107,9 @@ __host__ __device__ inline MlpPackLayout mlp_pack_layout(const K4Dev& s) {
     return L;
 }
 
-template <int MODE>
+// ACT: the hidden activation (K4_ACT_*, RgbAct in k4_march_common.cuh), applied to the fp32 accumulators before they
+// are rounded (F16) or split (F16X3) into the next layer's fp16 A fragments.
+template <int MODE, int ACT = K4_ACT_RELU>
 struct MmaWarpCtx {
     static constexpr bool kX3 = (MODE == K4_MLP_F16X3);
     static constexpr int kParts = kX3 ? 2 : 1;
@@ -344,7 +346,7 @@ struct MmaWarpCtx {
                         for (int m = 0; m < MT; ++m) {
                             float v[8];
 #pragma unroll
-                            for (int q = 0; q < 4; ++q) { v[q] = fmaxf(acc[m][0][q], 0.f); v[4 + q] = fmaxf(acc[m][1][q], 0.f); }
+                            for (int q = 0; q < 4; ++q) { v[q] = RgbAct<ACT>::tc(acc[m][0][q], s.act_c); v[4 + q] = RgbAct<ACT>::tc(acc[m][1][q], s.act_c); }
                             if constexpr (kX3) {
                                 split_h2(v[0], v[1], h1h[m][np][0], h1l[m][np][0]);
                                 split_h2(v[2], v[3], h1h[m][np][1], h1l[m][np][1]);
@@ -402,7 +404,7 @@ struct MmaWarpCtx {
                             }
                         }
                     }
-                    // ReLU, repack as the k16 A fragment `np` of layer 3, and consume it at once
+                    // activation, repack as the k16 A fragment `np` of layer 3, and consume it at once
                     const uint32_t off3 = (uint32_t)(L.off_w[2] + (((lane & 7)) * L.kstride[2] + np * 16 + ((lane >> 3) & 1) * 8) * 2);
                     uint32_t b3h[2], b3l[2];
                     ldsm_x2(smem_u32(w_part[0]) + off3, b3h[0], b3h[1]);
@@ -411,7 +413,7 @@ struct MmaWarpCtx {
                     for (int m = 0; m < MT; ++m) {
                         float v[8];
 #pragma unroll
-                        for (int q = 0; q < 4; ++q) { v[q] = fmaxf(acc[m][0][q], 0.f); v[4 + q] = fmaxf(acc[m][1][q], 0.f); }
+                        for (int q = 0; q < 4; ++q) { v[q] = RgbAct<ACT>::tc(acc[m][0][q], s.act_c); v[4 + q] = RgbAct<ACT>::tc(acc[m][1][q], s.act_c); }
                         uint32_t ah[4], al[4];
                         if constexpr (kX3) {
                             split_h2(v[0], v[1], ah[0], al[0]); split_h2(v[2], v[3], ah[1], al[1]);
@@ -458,8 +460,8 @@ struct MmaWarpCtx {
 };
 
 // fp32 mode: the context is an empty shell.
-template <>
-struct MmaWarpCtx<K4_MLP_FP32> {
+template <int ACT>
+struct MmaWarpCtx<K4_MLP_FP32, ACT> {
     int n_batches;
     __host__ __device__ static bool supported(const K4Dev&) { return true; }
     __host__ __device__ static size_t smem_bytes(const K4Dev&) { return 0; }

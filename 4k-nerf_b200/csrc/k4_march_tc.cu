@@ -84,7 +84,8 @@ struct TcRay {
     float t_min, t_max;
 };
 
-template <class Cfg>
+// ACT: the rgbnet's hidden activation (K4_ACT_*); CfgB, the DirectMPIGO shape, is also built with gauss and lkrelu.
+template <class Cfg, int ACT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k4_march_tc_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4RenderParams rp) {
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -131,7 +132,8 @@ k4_march_tc_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
         asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");      // generic smem writes -> async proxy
         wg_bar(wg);
         if (wt == 0) ++n_batches;
-        mlp_batch_wgmma<W, KPAD, true>(a_tile, blob, BL, valid, head & (TC_RING - 1), qw, qowner, nullptr, racc, wt, [] {}, true);
+        mlp_batch_wgmma<W, KPAD, true, ACT>(a_tile, blob, BL, valid, head & (TC_RING - 1), qw, qowner, nullptr, racc, wt, s.act_c,
+                                            [] {}, true);
     };
 
     for (unsigned iter = 0;; ++iter) {
@@ -358,9 +360,9 @@ k4_march_tc_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
     }
 }
 
-template <class Cfg>
+template <class Cfg, int ACT = K4_ACT_RELU>
 int launch_tc(const k4_scene* sc, K4RenderParams rp, cudaStream_t st) {
-    auto kern = k4_march_tc_kernel<Cfg>;
+    auto kern = k4_march_tc_kernel<Cfg, ACT>;
     K4_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
     int dev = 0, sms = 0;
     K4_CUDA_TRY(cudaGetDevice(&dev));
@@ -390,6 +392,10 @@ bool matches(const K4Dev& v) {
 bool k4_tc_supported(const K4Dev& v) { return matches<CfgA>(v) || matches<CfgB>(v); }
 
 int k4_launch_march_tc(const k4_scene* sc, K4RenderParams rp, cudaStream_t st) {
+    if (sc->act != K4_ACT_RELU) {           // DirectMPIGO only (k4_scene_create)
+        if (!matches<CfgB>(sc->dev)) return K4_ERR_UNSUPPORTED;
+        return sc->act == K4_ACT_GAUSS ? launch_tc<CfgB, K4_ACT_GAUSS>(sc, rp, st) : launch_tc<CfgB, K4_ACT_LKRELU>(sc, rp, st);
+    }
     if (matches<CfgA>(sc->dev)) return launch_tc<CfgA>(sc, rp, st);
     if (matches<CfgB>(sc->dev)) return launch_tc<CfgB>(sc, rp, st);
     return K4_ERR_UNSUPPORTED;

@@ -119,8 +119,9 @@ struct WgCtl {
 };
 
 // PROF: the profiled instantiation (k4_testing_march_phases).  It adds the phase marks of PhaseClock and nothing else, and
-// writes each warpgroup's counters to phases[(blockIdx.x * 4 + wg) * K4_PHASE_SLOTS ..].
-template <class Cfg, bool PROF>
+// writes each warpgroup's counters to phases[(blockIdx.x * 4 + wg) * K4_PHASE_SLOTS ..].  ACT: the rgbnet's hidden
+// activation (K4_ACT_*); the DirectMPIGO configs are also built with gauss and lkrelu, the profiled kernel with relu only.
+template <class Cfg, int ACT, bool PROF>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4RenderParams rp, unsigned long long* phases) {
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -183,11 +184,11 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
             const int valid = *reinterpret_cast<volatile int*>(&c->valid[tile]);
             const bool last = *reinterpret_cast<volatile int*>(&c->last[tile]) != 0;
             if (PROF)
-                mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0>(ring_s + tile * Cfg::TILE_BYTES, blob, BL, valid, tile * 128u, qw, qowner,
-                                                           qdiff, racc, wt, consumed, last, clk);
+                mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0, ACT>(ring_s + tile * Cfg::TILE_BYTES, blob, BL, valid, tile * 128u, qw,
+                                                                qowner, qdiff, racc, wt, s.act_c, consumed, last, clk);
             else
-                mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0>(ring_s + tile * Cfg::TILE_BYTES, blob, BL, valid, tile * 128u, qw, qowner,
-                                                           qdiff, racc, wt, consumed, last);
+                mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0, ACT>(ring_s + tile * Cfg::TILE_BYTES, blob, BL, valid, tile * 128u, qw,
+                                                                qowner, qdiff, racc, wt, s.act_c, consumed, last);
             ++nb;
         }
         if (rp.counters && wt == 0) atomicAdd(rp.counters + 3, n_batches);
@@ -528,11 +529,16 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
 }
 
 // phases: NULL for the production kernel, else the profiled one writes there (room for max_ctas CTAs); *n_ctas: CTAs launched
-template <class Cfg>
+template <class Cfg, int ACT>
 int launch_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st, unsigned long long* phases, int max_ctas, int* n_ctas) {
     if (sc->dev.Cpad != Cfg::CPAD) return K4_ERR_UNSUPPORTED;     // the k0 gather's stride is the config's
-    auto kern = phases ? k4_march_ws_kernel<Cfg, true> : k4_march_ws_kernel<Cfg, false>;
-    const int smem = phases ? Cfg::PROF_SMEM : Cfg::SMEM;
+    auto kern = k4_march_ws_kernel<Cfg, ACT, false>;
+    int smem = Cfg::SMEM;
+    if constexpr (ACT == K4_ACT_RELU) {
+        if (phases) { kern = k4_march_ws_kernel<Cfg, ACT, true>; smem = Cfg::PROF_SMEM; }
+    } else if (phases) {
+        return K4_ERR_UNSUPPORTED;                              // the profiled kernel is built with relu only
+    }
     int dev = 0, sms = 0;
     K4_CUDA_TRY(cudaGetDevice(&dev));
     K4_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -552,7 +558,7 @@ int launch_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st, unsigned l
 // k4_testing_rgbnet, wgmma modes: one CTA = one warpgroup = one batch of up to 128 caller rows.  The operand blob is staged
 // as the marchers stage it; row r goes to ring-tile row r through the scene's column map (pack2, other columns zero), its
 // weight / owner / diffuse logits to the queue, and mlp_batch_wgmma accumulates the colours into racc.
-template <class Cfg>
+template <class Cfg, int ACT>
 __global__ void __launch_bounds__(TC_WG, 1)
 k4_test_rgbnet_ws_kernel(const __grid_constant__ K4Dev s, const float* __restrict__ xs, const float* __restrict__ diffs,
                          const float* __restrict__ ws, const int* __restrict__ owners, long long n, float* __restrict__ racc_out) {
@@ -601,15 +607,15 @@ k4_test_rgbnet_ws_kernel(const __grid_constant__ K4Dev s, const float* __restric
     asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");      // generic smem writes -> async proxy
     tc_mbar_wait(bar, 0);
     __syncthreads();
-    mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0>(s_u32(tile), blob, BL, valid, 0u, qw, qowner, qdiff, racc, wt, [] {}, true);
+    mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0, ACT>(s_u32(tile), blob, BL, valid, 0u, qw, qowner, qdiff, racc, wt, s.act_c, [] {}, true);
     __syncthreads();
 #pragma unroll
     for (int c = 0; c < 3; ++c) racc_out[3 * (r0 + wt) + c] = racc[3 * wt + c];
 }
 
-template <class Cfg>
+template <class Cfg, int ACT>
 int launch_test_rgbnet_ws(const k4_scene* sc, const k4_rgbnet_test_args* a, cudaStream_t st) {
-    auto kern = k4_test_rgbnet_ws_kernel<Cfg>;
+    auto kern = k4_test_rgbnet_ws_kernel<Cfg, ACT>;
     constexpr int smem = Cfg::BLOB_PAD + Cfg::TILE_BYTES + TC_WG * (4 + 12 + 12 + 1) + 16;
     K4_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     const long long blocks = (a->n + TC_WG - 1) / TC_WG;
@@ -618,12 +624,33 @@ int launch_test_rgbnet_ws(const k4_scene* sc, const k4_rgbnet_test_args* a, cuda
     return K4_OK;
 }
 
+// The instantiation of a config for the scene's activation: relu for every config, gauss and lkrelu for the DirectMPIGO
+// ones (the only kind whose reference builds them).
+template <class Cfg>
+int launch_ws_act(const k4_scene* sc, K4RenderParams rp, cudaStream_t st, unsigned long long* phases, int max_ctas, int* n_ctas) {
+    if constexpr (Cfg::KIND == K4_KIND_DMPIGO) {
+        if (sc->act == K4_ACT_GAUSS) return launch_ws<Cfg, K4_ACT_GAUSS>(sc, rp, st, phases, max_ctas, n_ctas);
+        if (sc->act == K4_ACT_LKRELU) return launch_ws<Cfg, K4_ACT_LKRELU>(sc, rp, st, phases, max_ctas, n_ctas);
+    }
+    if (sc->act != K4_ACT_RELU) return K4_ERR_UNSUPPORTED;
+    return launch_ws<Cfg, K4_ACT_RELU>(sc, rp, st, phases, max_ctas, n_ctas);
+}
+template <class Cfg>
+int launch_test_rgbnet_ws_act(const k4_scene* sc, const k4_rgbnet_test_args* a, cudaStream_t st) {
+    if constexpr (Cfg::KIND == K4_KIND_DMPIGO) {
+        if (sc->act == K4_ACT_GAUSS) return launch_test_rgbnet_ws<Cfg, K4_ACT_GAUSS>(sc, a, st);
+        if (sc->act == K4_ACT_LKRELU) return launch_test_rgbnet_ws<Cfg, K4_ACT_LKRELU>(sc, a, st);
+    }
+    if (sc->act != K4_ACT_RELU) return K4_ERR_UNSUPPORTED;
+    return launch_test_rgbnet_ws<Cfg, K4_ACT_RELU>(sc, a, st);
+}
+
 }  // namespace
 
 int k4_testing_rgbnet_ws(const k4_scene* sc, const k4_rgbnet_test_args* a, cudaStream_t st) {
     if (!sc->dev.tc_blob || !sc->dev.tc_colmap) return K4_ERR_UNSUPPORTED;
     switch (sc->dev.tc_cfg) {
-#define K4_X(id, kind, C, vpe, spe, W, direct) case id: return launch_test_rgbnet_ws<TcCfg<id, kind, C, vpe, spe, W, direct>>(sc, a, st);
+#define K4_X(id, kind, C, vpe, spe, W, direct) case id: return launch_test_rgbnet_ws_act<TcCfg<id, kind, C, vpe, spe, W, direct>>(sc, a, st);
         K4_WS_CFG_LIST(K4_X)
 #undef K4_X
         default: return K4_ERR_UNSUPPORTED;
@@ -634,7 +661,7 @@ int k4_launch_march_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st, u
     if (!sc->dev.tc_blob) return K4_ERR_UNSUPPORTED;
     switch (sc->dev.tc_cfg) {
 #define K4_X(id, kind, C, vpe, spe, W, direct) \
-        case id: return launch_ws<TcCfg<id, kind, C, vpe, spe, W, direct>>(sc, rp, st, phases, max_ctas, n_ctas);
+        case id: return launch_ws_act<TcCfg<id, kind, C, vpe, spe, W, direct>>(sc, rp, st, phases, max_ctas, n_ctas);
         K4_WS_CFG_LIST(K4_X)
 #undef K4_X
         default: return K4_ERR_UNSUPPORTED;

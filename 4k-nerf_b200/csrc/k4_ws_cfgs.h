@@ -3,9 +3,12 @@
 // config a model runs on).
 //
 // A model does not need a config of exactly its own shape: a config COVERS every model of the same kind / direct-ness
-// with at most as many k0 channels, view / position frequencies and hidden units, because the missing inputs and units
-// are exact zeros in the packed operands (zero weight columns for inputs the model does not have, zero rows / columns
-// for hidden units it does not have: relu(0) = 0 contributes nothing).  The first covering config in list order is used,
+// with at most as many k0 channels, view / position frequencies and hidden units.  The config's extra inputs meet zero
+// weight columns.  A hidden unit the model does not have has zero incoming weights and bias, so its pre-activation is 0,
+// but its activated value need not be (gauss(0) = 1): what makes it contribute nothing is that its OUTGOING weights --
+// its column of W2 or W3 -- are exact zeros in the packed blob (k4_scene_create zeroes the blob and writes only the
+// model's own rows and columns).  The fp32 and mma.sync packs never hold such units: their widths are the model's own,
+// and the fp32 pack's padded columns (ldw > n_out) are computed but never read as inputs.  The first covering config in list order is used,
 // so the list goes from cheap to expensive within a kind.  Shapes of the shipped reference configs come first:
 //   configs/default.py:107-119            DVGO   k0 12, viewbase_pe 4 (ctor default lib/dvgo.py:33), width 128, direct
 //   configs/syn/1x_chair_joint_l1+gan.py  DVGO   k0 12, viewbase_pe 0, width 128, direct

@@ -7,7 +7,7 @@ memory, streams and ``torch.distributed`` only; every hot op is a hand-written s
 There is NO CPU fallback: a missing library or CPU tensors raise.
 """
 from . import _lib  # noqa: F401  (fails loudly if libk4nerf.so is missing)
-from . import grid, dvgo, dmpigo, dcvgo, utils, render, sr_esrnet, masked_adam  # noqa: F401
+from . import act, grid, dvgo, dmpigo, dcvgo, utils, render, sr_esrnet, masked_adam  # noqa: F401
 from .masked_adam import MaskedAdam  # noqa: F401
 from .dvgo import DirectVoxGO, get_rays_of_a_view  # noqa: F401
 from .dmpigo import DirectMPIGO  # noqa: F401
@@ -15,4 +15,4 @@ from .dcvgo import DirectContractedVoxGO  # noqa: F401
 from .sr_esrnet import SFTNet  # noqa: F401
 
 __all__ = ['DirectVoxGO', 'DirectMPIGO', 'DirectContractedVoxGO', 'SFTNet', 'get_rays_of_a_view', 'grid', 'dvgo', 'dmpigo', 'utils', 'render',
-           'sr_esrnet']
+           'sr_esrnet', 'act']

@@ -8,6 +8,7 @@ LIB_PATH = os.path.join(_HERE, 'libk4nerf.so')
 K4_OK = 0
 K4_KIND_DVGO, K4_KIND_DMPIGO, K4_KIND_DCVGO = 0, 1, 2
 K4_MLP_FP32, K4_MLP_F16, K4_MLP_F16X3, K4_MLP_TCGEN05, K4_MLP_TCGEN05_WS = 0, 1, 2, 3, 4
+K4_ACT_RELU, K4_ACT_GAUSS, K4_ACT_LKRELU = 0, 1, 2
 K4_MAX_MLP_LAYERS = 8
 K4_MAX_PEERS = 8
 MLP_MODES = {'fp32': K4_MLP_FP32, 'f16': K4_MLP_F16, 'f16x3': K4_MLP_F16X3, 'tcgen05': K4_MLP_TCGEN05,
@@ -23,10 +24,11 @@ class SceneDesc(C.Structure):
         ('fast_color_thres', C.c_float),
         ('max_world_size', C.c_int32), ('mpi_depth', C.c_int32),
         ('rgbnet_depth', C.c_int32), ('rgbnet_width', C.c_int32), ('rgbnet_direct', C.c_int32),
-        ('viewbase_pe', C.c_int32), ('spatial_pe', C.c_int32), ('reserved0', C.c_int32),
+        ('viewbase_pe', C.c_int32), ('spatial_pe', C.c_int32), ('rgbnet_act', C.c_int32),
         ('d_density', C.c_void_p), ('d_k0', C.c_void_p), ('d_mask', C.c_void_p), ('d_act_shift_grid', C.c_void_p),
         ('d_rgbnet_weight', C.c_void_p * K4_MAX_MLP_LAYERS), ('d_rgbnet_bias', C.c_void_p * K4_MAX_MLP_LAYERS),
         ('scene_center', C.c_float * 3), ('scene_radius', C.c_float * 3), ('bg_len', C.c_float), ('world_len', C.c_int32),
+        ('rgbnet_act_param', C.c_float),
     ]
 
 

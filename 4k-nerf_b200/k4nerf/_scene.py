@@ -58,7 +58,7 @@ def scalar_fingerprint(module, extra):
     """Scalars baked into the device scene (k4_scene_desc): a change must rebuild it."""
     return (float(module.fast_color_thres), host_float(module, 'voxel_size_ratio'), float(extra.get('act_shift', 0.0)),
             float(extra.get('voxel_size', 0.0)), int(extra.get('viewbase_pe', 0)), int(extra.get('spatial_pe', 0)),
-            bool(extra.get('rgbnet_direct', True)))
+            bool(extra.get('rgbnet_direct', True)), int(extra.get('rgbnet_act', _lib.K4_ACT_RELU)))
 
 
 def require_cuda(*tensors):
@@ -84,6 +84,8 @@ def gather_tensors(module, extra):
     tensors += [p for l in layers for p in (l.weight, l.bias)]
     if extra.get('act_shift_grid') is not None:
         tensors.append(extra['act_shift_grid'])
+    if extra.get('rgbnet_act_param') is not None:
+        tensors.append(extra['rgbnet_act_param'])
     return tensors
 
 
@@ -117,6 +119,9 @@ def build_scene(kind, module, extra):
     d.rgbnet_direct = int(bool(extra.get('rgbnet_direct', True)))
     d.viewbase_pe = int(extra.get('viewbase_pe', 0))
     d.spatial_pe = int(extra.get('spatial_pe', 0))
+    d.rgbnet_act = int(extra.get('rgbnet_act', _lib.K4_ACT_RELU))
+    if extra.get('rgbnet_act_param') is not None:
+        d.rgbnet_act_param = float(extra['rgbnet_act_param'])      # GaussianActivation.a, read when the scene is built
     if 'scene_center' in extra:
         d.scene_center[:] = extra['scene_center']
         d.scene_radius[:] = extra['scene_radius']

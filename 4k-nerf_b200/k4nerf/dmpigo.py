@@ -5,6 +5,20 @@ import torch
 import torch.nn as nn
 
 from . import _lib, grid
+from .act import GaussianActivation
+
+# act_type -> the module after every hidden nn.Linear of the rgbnet (lib/dmpigo.py:89-95) and its K4_ACT_* code
+_ACT_TYPES = {'relu': _lib.K4_ACT_RELU, 'gauss': _lib.K4_ACT_GAUSS, 'lkrelu': _lib.K4_ACT_LKRELU}
+
+
+def make_act(act_type):
+    if act_type == 'relu':
+        return nn.ReLU(inplace=True)
+    if act_type == 'gauss':
+        return GaussianActivation(a=0.05)
+    if act_type == 'lkrelu':
+        return nn.LeakyReLU()
+    raise ValueError(f"act_type must be one of 'relu', 'gauss', 'lkrelu', not {act_type!r}")
 from ._scene import FusedRenderMixin
 from .maintain import GridMaintenanceMixin
 from .coarse import CoarseStageMixin
@@ -55,8 +69,6 @@ class DirectMPIGO(FusedRenderMixin, GridMaintenanceMixin, CoarseStageMixin, nn.M
             self.k0_dim = 3
             self.rgbnet = None
         else:
-            if self.act_type != 'relu':
-                raise NotImplementedError("only act_type='relu' (the shipped configs) is built")
             if self.mode_type in ('TRANS', 'adain'):
                 raise NotImplementedError('mode_type TRANS/adain need modules the reference does not ship')
             self.k0_dim = rgbnet_dim
@@ -64,7 +76,7 @@ class DirectMPIGO(FusedRenderMixin, GridMaintenanceMixin, CoarseStageMixin, nn.M
             self.register_buffer('posfreq', torch.FloatTensor([(2 ** i) for i in range(spatial_pe)]))
             self.dim0 = (3 + 3 * viewbase_pe * 2 + 3 + 3 * spatial_pe * 2) + self.k0_dim
             self.pe_dim = 3 + 3 * viewbase_pe * 2 + 3 + 3 * spatial_pe * 2
-            act = nn.ReLU(inplace=True)
+            act = make_act(self.act_type)      # ONE instance after every hidden Linear, as the reference shares it
             self.rgbnet = nn.Sequential(
                 nn.Linear(self.dim0, rgbnet_width), act,
                 *[nn.Sequential(nn.Linear(rgbnet_width, rgbnet_width), act) for _ in range(rgbnet_depth - 2)],
@@ -136,4 +148,6 @@ class DirectMPIGO(FusedRenderMixin, GridMaintenanceMixin, CoarseStageMixin, nn.M
             'mpi_depth': int(self.mpi_depth), 'act_shift_grid': self.act_shift.grid.detach(),
             'viewbase_pe': self.viewbase_pe if self.rgbnet is not None else 0,
             'spatial_pe': self.spatial_pe if self.rgbnet is not None else 0,
+            'rgbnet_act': _ACT_TYPES[self.act_type] if self.rgbnet is not None else _lib.K4_ACT_RELU,
+            'rgbnet_act_param': self.rgbnet[1].a.detach() if self.rgbnet is not None and self.act_type == 'gauss' else None,
         }

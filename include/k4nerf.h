@@ -57,6 +57,17 @@ enum { K4_MLP_FP32 = 0,                    /* fp32 FFMA, sequential accumulation
        K4_MLP_TCGEN05 = 3,                 /* wgmma, fp16 operands (warpgroup-wide batches)      */
        K4_MLP_TCGEN05_WS = 4 };            /* same, MLP in its own warpgroup (warp-specialised)  */
 
+/* The colour MLP's hidden activation (DirectMPIGO's fine_model_and_render.act_type, lib/dmpigo.py:89-95): the
+ * module after every hidden nn.Linear.  DirectVoxGO and DirectContractedVoxGO always use K4_ACT_RELU.
+ *   K4_ACT_RELU    max(x, 0)
+ *   K4_ACT_GAUSS   exp(-x^2 / (2 a^2)), GaussianActivation (lib/act.py), a = k4_scene_desc.rgbnet_act_param
+ *   K4_ACT_LKRELU  x > 0 ? x : 0.01 x (nn.LeakyReLU())
+ * Every mode evaluates the activation in fp32 on the layer's fp32 result.  fp32 mode follows torch's expression
+ * order (gauss: expf(-(x*x) / (2*(a*a))), division and expf as torch does them); the tensor-core modes take
+ * ex2.approx(x*x*c) with c = -log2(e) / (2 a^2) rounded once from double, and round the activated value to fp16 as
+ * they round a ReLU'd one. */
+enum { K4_ACT_RELU = 0, K4_ACT_GAUSS = 1, K4_ACT_LKRELU = 2 };
+
 #define K4_MAX_MLP_LAYERS 8
 #define K4_MAX_PEERS 8            /* GPUs of one NVLink / NVSwitch node */
 
@@ -89,7 +100,7 @@ typedef struct k4_scene_desc {
     int32_t rgbnet_direct;        /* DVGO only (lib/dvgo.py:382-386,409-412)                    */
     int32_t viewbase_pe;          /* number of view-direction frequencies                       */
     int32_t spatial_pe;           /* MPI only: number of positional frequencies                 */
-    int32_t reserved0;
+    int32_t rgbnet_act;           /* K4_ACT_*; MPI only, every other kind must keep K4_ACT_RELU  */
     const float* d_density;       /* [X*Y*Z]                                                    */
     const float* d_k0;            /* [C*X*Y*Z] planar, reference layout                         */
     const uint8_t* d_mask;        /* [mX*mY*mZ] bytes, non-zero = occupied                      */
@@ -101,6 +112,7 @@ typedef struct k4_scene_desc {
     float scene_radius[3];        /* (xyz_max - xyz_min) / 2                                     */
     float bg_len;                 /* thickness of the contracted background shell                */
     int32_t world_len;            /* world_size[0]                                               */
+    float rgbnet_act_param;       /* K4_ACT_GAUSS: the Gaussian's a (finite, > 0); ignored otherwise */
 } k4_scene_desc;
 
 /* render_kwargs of the reference forward (run_sr.py:1311-1320; lib/dvgo.py:327) + kernel knobs. */
