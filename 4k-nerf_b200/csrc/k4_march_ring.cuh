@@ -1,0 +1,164 @@
+// k4_march_ring.cuh -- what the two wgmma marchers (k4_march_tc.cu, k4_march_ws.cu) share beyond k4_march_ray.cuh:
+// the PTX helpers, the config (derived constants and shared-memory map), the TMA staging of the operand blob, the packed
+// view embedding of a ray and the features of a surviving sample.  Each kernel reserves ring rows and stores them itself:
+// k4_march_ws.cu packs a row chunk by chunk with the view words read from shared memory to stay under its 128 registers,
+// k4_march_tc.cu builds the row in registers.
+#pragma once
+#include "k4_internal.cuh"
+#include "k4_march_common.cuh"
+#include "k4_march_mlp.cuh"
+
+namespace {
+
+constexpr int TC_WG = 128;           // threads of a warpgroup = rays of a tile = rows of an MLP batch
+constexpr int TC_ROUND = 8;          // marching steps between warpgroup rendezvous when nothing is pending
+
+// ---------------------------------------------------------------------------------------------
+// PTX helpers
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" :: "r"(s_u32(bar)), "r"(count));
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+    uint32_t ok = 0;
+    while (!ok) {
+        asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n"
+                     : "=r"(ok) : "r"(s_u32(bar)), "r"(parity) : "memory");
+    }
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" :: "r"(s_u32(bar)) : "memory");
+}
+__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
+    uint32_t ok;
+    asm volatile("{\n.reg .pred p;\nmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n"
+                 : "=r"(ok) : "r"(s_u32(bar)), "r"(parity) : "memory");
+    return ok != 0;
+}
+__device__ __forceinline__ uint32_t pack2(float lo, float hi) {
+    uint32_t d;      // saturating: a feature beyond the fp16 range becomes +-65504, never inf
+    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;\n" : "=r"(d) : "f"(hi), "f"(lo));
+    return d;
+}
+// named barrier `id` over the 128 threads of a warpgroup (marcher group wg uses id wg + 1; 0 is __syncthreads), and its
+// form that also ORs a predicate over them
+__device__ __forceinline__ void named_bar(int id) { asm volatile("bar.sync %0, 128;\n" :: "r"(id) : "memory"); }
+__device__ __forceinline__ bool named_bar_or(int id, bool pred) {
+    uint32_t r;
+    asm volatile("{\n.reg .pred p, q;\nsetp.ne.u32 p, %2, 0;\nbarrier.cta.red.or.pred q, %1, 128, p;\nselp.u32 %0, 1, 0, q;\n}\n"
+                 : "=r"(r) : "r"(id), "r"((uint32_t)pred) : "memory");
+    return r != 0;
+}
+
+// The operand blob (weights + bias tiles) from global to shared memory as one TMA bulk copy that completes on `bar`.
+// One thread calls it, once bar's mbarrier.init is visible; everybody then waits for phase 0 of bar.
+__device__ __forceinline__ void stage_blob(unsigned char* blob, const void* src, int bytes, uint64_t* bar) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" :: "r"(s_u32(bar)), "r"((uint32_t)bytes) : "memory");
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
+                 :: "r"(s_u32(blob)), "l"(src), "r"((uint32_t)bytes), "r"(s_u32(bar)) : "memory");
+}
+
+// ---------------------------------------------------------------------------------------------
+// A model shape one of the kernels is built for: an entry of K4_WS_CFG_LIST (k4_ws_cfgs.h) for k4_march_ws.cu, CfgA /
+// CfgB (ID -1) for k4_march_tc.cu.  Row layout of the A operand (fp16): [per-sample features: k0 channels K0OFF..C-1, MPI
+// position + its sin/cos, zero-padded to an even count NS][view embedding: v, sin, cos (NVEMB)][zeros to KPAD].
+// TILES: 128-row tiles of a marcher group's ring.  VWS: the marcher keeps its ray's packed view embedding in shared
+// memory (WG_VW) rather than in registers.
+// ---------------------------------------------------------------------------------------------
+template <int ID_, int KIND_, int C_, int VIEWPE_, int SPAPE_, int W_, int DIRECT_, int TILES_, bool VWS_>
+struct TcCfg {
+    static constexpr int ID = ID_, KIND = KIND_, C = C_, VIEWPE = VIEWPE_, SPAPE = SPAPE_, W = W_, DIRECT = DIRECT_;
+    static constexpr int TILES = TILES_, RING = TILES * 128;
+    static constexpr bool VWS = VWS_;
+    static constexpr int CPAD = (C + 3) & ~3;
+    static constexpr int NVEMB = 3 + 6 * VIEWPE;
+    static constexpr int NPOS = (KIND == K4_KIND_DMPIGO) ? 3 + 6 * SPAPE : 0;
+    static constexpr int K0OFF = DIRECT ? 0 : 3;        // rgbnet_direct=False: k0[0:3] is the diffuse logit (lib/dvgo.py:385-386,412)
+    static constexpr int NS0 = C - K0OFF + NPOS;        // per-sample features
+    static constexpr int NS = (NS0 + 1) & ~1;           // ... padded to an even count (rows are packed as fp16 pairs)
+    static constexpr int NF = ((CPAD > C + NPOS) ? CPAD : C + NPOS) + 1;   // feature scratch (k0 quads, position code, pad)
+    static constexpr int DIM0 = NS + NVEMB;
+    static constexpr int KPAD = (DIM0 + 15) & ~15;
+    static constexpr int KCH = KPAD / 8;                // 16-byte chunks per A row
+    static constexpr int NVW = (NVEMB + 1) / 2;         // packed per-ray words
+    static constexpr int TILE_BYTES = 128 * KPAD * 2;
+    static_assert(W == 128 || W == 64, "hidden width");
+    static_assert(DIRECT || KIND == K4_KIND_DVGO, "the diffuse term exists in DirectVoxGO only");
+    // shared memory map: [blob][marcher group 0][marcher group 1][weight mbarrier]; offsets WG_* inside a group's block
+    static constexpr int BLOB = W * KPAD * 2 + W * W * 2 + 16 * W * 2 + 2 * W * 16 * 2 + 16 * 16 * 2 + 128 * 16 * 2;
+    static constexpr int BLOB_PAD = (BLOB + 1023) & ~1023;
+    static constexpr int WG_A = TILES * TILE_BYTES;
+    static constexpr int WG_QW = WG_A;                       // float[RING]
+    static constexpr int WG_RACC = WG_QW + RING * 4;         // float[128*3]
+    static constexpr int WG_OWNER = WG_RACC + 128 * 3 * 4;   // u8[RING]
+    static constexpr int WG_QDIFF = WG_OWNER + RING;         // float[RING*3]: diffuse logits of the queued samples (!DIRECT only)
+    static constexpr int WG_VW = WG_QDIFF + (DIRECT ? 0 : RING * 3 * 4);     // u32[NVW][128]: packed view embedding per ray (VWS only)
+    static constexpr int WG_MISC = WG_VW + (VWS ? NVW * 128 * 4 : 0);        // the kernel's control block: tail first, then its own
+    static constexpr int WG_BYTES = (WG_MISC + 128 + 1023) & ~1023;
+    static constexpr int CTA_MISC = BLOB_PAD + 2 * WG_BYTES; // weight mbarrier
+    static constexpr int SMEM = CTA_MISC + 64;
+    static constexpr int PROF_SMEM = SMEM + 4 * PhaseClock::WORDS * 8;   // + the phase counters of a profiled kernel
+    static_assert(PROF_SMEM <= 227 * 1024, "shared memory of one block");
+};
+
+// ---------------------------------------------------------------------------------------------
+// per ray
+// ---------------------------------------------------------------------------------------------
+// view-direction embedding, packed once per ray into NVW fp16 pairs (lib/dvgo.py:387-388)
+template <class Cfg>
+__device__ __forceinline__ void pack_view_embedding(Vec3 v, uint32_t vw[Cfg::NVW]) {
+    float ve[Cfg::NVEMB + 1];
+    const float vv[3] = {v.x, v.y, v.z};
+    ve[0] = vv[0]; ve[1] = vv[1]; ve[2] = vv[2];
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+#pragma unroll
+        for (int f = 0; f < Cfg::VIEWPE; ++f) {
+            const float a = __fmul_rn(vv[c], (float)(1 << f));
+            ve[3 + c * Cfg::VIEWPE + f] = sinf(a);
+            ve[3 + 3 * Cfg::VIEWPE + c * Cfg::VIEWPE + f] = cosf(a);
+        }
+    ve[Cfg::NVEMB] = 0.f;
+#pragma unroll
+    for (int j = 0; j < Cfg::NVW; ++j) vw[j] = pack2(ve[2 * j], ve[2 * j + 1]);
+}
+
+// ---------------------------------------------------------------------------------------------
+// per surviving sample
+// ---------------------------------------------------------------------------------------------
+// f[0..C): the k0 features; behind them DirectMPIGO's position code (lib/dmpigo.py:338,347-351); a zero where the row's
+// feature count is odd.  The row takes f[K0OFF ..].
+template <class Cfg>
+__device__ __forceinline__ void sample_features(const K4Dev& s, const Cell& cell, const float cw[8], const int cidx[8], float f[Cfg::NF]) {
+    interp_k0_cfg<Cfg::CPAD / 4>(s, cw, cidx, f);       // f[0..C) (CPAD >= C; extra lanes unused)
+    if (Cfg::KIND == K4_KIND_DMPIGO) {
+        const float pe[3] = {cell.cz, cell.cy, cell.cx};   // .flip(-1)
+        f[Cfg::C + 0] = pe[0]; f[Cfg::C + 1] = pe[1]; f[Cfg::C + 2] = pe[2];
+#pragma unroll
+        for (int c = 0; c < 3; ++c)
+#pragma unroll
+            for (int q = 0; q < Cfg::SPAPE; ++q) {
+                const float a = __fmul_rn(pe[c], (float)(1 << q));
+                f[Cfg::C + 3 + c * Cfg::SPAPE + q] = sinf(a);
+                f[Cfg::C + 3 + 3 * Cfg::SPAPE + c * Cfg::SPAPE + q] = cosf(a);
+            }
+    }
+    if (Cfg::NS0 & 1) f[Cfg::K0OFF + Cfg::NS0] = 0.f;          // pad column of an odd feature count
+}
+
+// ---------------------------------------------------------------------------------------------
+// launch geometry of the persistent wgmma marchers: 128-ray tiles (16x8 pixels of an image, or 128 consecutive rays), two
+// marcher groups per CTA, at most one CTA per SM.  Sets rp.n_tiles, returns the number of CTAs.
+// ---------------------------------------------------------------------------------------------
+inline long long wg_launch_geometry(K4RenderParams& rp, int sms) {
+    if (rp.image_w > 0) rp.n_tiles = (long long)((rp.image_w + 15) / 16) * ((rp.image_h + 7) / 8);
+    else rp.n_tiles = (rp.n_rays + TC_WG - 1) / TC_WG;
+    long long blocks = (rp.n_tiles + 1) / 2;
+    if (blocks > sms) blocks = sms;                     // persistent: one CTA per SM
+    if (blocks < 1) blocks = 1;
+    return blocks;
+}
+
+}  // namespace
