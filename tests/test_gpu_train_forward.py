@@ -1,9 +1,8 @@
 """GPU: the training-side forward (k4nerf/train_forward.py, SURVEY.md section 8 f-2).
 
 (i) values: the per-sample lists and per-ray outputs against the oracle pipeline running on the
-reference's own kernels (oracle/_ref) on the same device; (ii) gradients: against a float64 pure-torch
-restatement of alpha / transmittance / compositing with autograd (no custom backward anywhere);
-(iii) a few MaskedAdam steps reduce the loss."""
+reference's own kernels (oracle/_ref) on the same device; (ii) a few MaskedAdam steps reduce the loss.
+The gradients are tested against a float64 restatement in test_gpu_train_grad.py."""
 import os
 
 import pytest
@@ -55,76 +54,6 @@ def test_sample_lists_match_reference_kernel_pipeline(ref_ops, cuda_device, name
     with torch.no_grad():
         fused = m(ro, rd, vd, **kw)
     assert pipeline.psnr(fused['rgb_marched'].cpu(), ours['rgb_marched'].cpu()) > 60
-
-
-def _float64_restatement(m, ro, rd, vd, kw):
-    """alpha / transmittance / compositing in float64 torch ops with plain autograd (DirectVoxGO)."""
-    from k4nerf import render_utils_cuda as rops
-    n = ro.shape[0]
-    stepdist = kw['stepsize'] * m.voxel_size
-    pts, outside, ray_id, step_id, *_ = rops.sample_pts_on_rays(ro, rd, m.xyz_min, m.xyz_max, kw['near'], 1e9, stepdist)
-    pts, ray_id = pts[~outside], ray_id[~outside]
-    occ = m.mask_cache(pts)
-    pts, ray_id = pts[occ], ray_id[occ]
-    interval = float(kw['stepsize'] * m.voxel_size_ratio)
-    den = m.density(pts).double()
-    alpha = 1 - (1 + torch.exp(den + float(m.act_shift))) ** (-interval)
-    sel = alpha.float() > m.fast_color_thres
-    pts, ray_id, alpha = pts[sel], ray_id[sel], alpha[sel]
-    log1m = torch.log1p(-alpha)
-    cs = torch.cumsum(log1m, 0)
-    excl = cs - log1m
-    first = torch.ones_like(ray_id, dtype=torch.bool)
-    first[1:] = ray_id[1:] != ray_id[:-1]
-    seg = torch.cumsum(first.long(), 0) - 1
-    T = torch.exp(excl - excl[first][seg])
-    live = (T.detach() >= 1e-3)
-    T_incl = T * (1 - alpha)
-    last_live = live.clone()
-    last_live[:-1] &= ~(live[1:] & ~first[1:])
-    alphainv_last = torch.ones(n, device=ro.device, dtype=torch.float64).index_put((ray_id[last_live],), T_incl[last_live])
-    weights = T * alpha * live
-    sel = weights.float() > m.fast_color_thres
-    pts, ray_id, weights = pts[sel], ray_id[sel], weights[sel]
-    k0 = m.k0(pts)
-    e = (vd.unsqueeze(-1) * m.viewfreq).flatten(-2)
-    vemb = torch.cat([vd, e.sin(), e.cos()], -1)[ray_id]
-    rgb = torch.sigmoid(m.rgbnet(torch.cat([k0, vemb], -1))).double()
-    rgb_marched = torch.zeros(n, 3, device=ro.device, dtype=torch.float64).index_add(0, ray_id, weights.unsqueeze(-1) * rgb)
-    return rgb_marched + alphainv_last.unsqueeze(-1) * kw['bg'], alphainv_last
-
-
-@pytest.mark.parametrize('regime', ['fog', 'shell'])
-def test_gradients_match_float64_autograd_restatement(cuda_device, regime):
-    dev = cuda_device
-    torch.backends.cuda.matmul.allow_tf32 = False
-    st = make_state('cfgA', res=24, regime=regime)
-    (ro, rd, vd), kw = rays_for(st, 20, 24)
-    ro, rd, vd = ro.to(dev), rd.to(dev), vd.to(dev)
-    g = torch.Generator().manual_seed(0)
-    target = torch.rand(ro.shape[0], 3, generator=g).to(dev)
-    grads = []
-    for which in ('ours', 'restatement'):
-        m = model_from_state(st, dev)
-        if which == 'ours':
-            out = m(ro, rd, vd, global_step=1, **kw)             # autograd enabled -> train_forward
-            assert 'weights' in out and out['rgb_marched'].requires_grad
-            rgb, last = out['rgb_marched'], out['alphainv_last']
-        else:
-            rgb, last = _float64_restatement(m, ro, rd, vd, kw)
-        loss = ((rgb - target) ** 2).mean() + 0.01 * (last ** 2).mean()
-        loss.backward()
-        grads.append({k: p.grad.detach().double().clone() for k, p in m.named_parameters() if p.grad is not None} | {'_loss': loss.detach().double()})
-    a, b = grads
-    assert abs(float(a['_loss'] - b['_loss'])) <= 1e-5 * max(1.0, abs(float(b['_loss'])))
-    assert set(a) == set(b) and {'density.grid', 'k0.grid', 'rgbnet.0.weight'} <= set(a)
-    for k in a:
-        if k == '_loss':
-            continue
-        scale = b[k].abs().max().item()
-        assert scale > 0, k
-        err = (a[k] - b[k]).abs().max().item()
-        assert err <= 2e-3 * scale, (k, err, scale)
 
 
 def test_masked_adam_training_steps_reduce_the_loss(cuda_device):
