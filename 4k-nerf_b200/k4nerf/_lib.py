@@ -174,7 +174,14 @@ EXPORTS = {
                                     C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     'k4_op_grid_sample_backward': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_float),
                                              C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
-    'k4_make_rays_rows': (C.c_int, [C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_int32,
+    'k4_op_distloss_workspace_bytes': (C.c_size_t, [C.c_int64]),
+    'k4_op_distloss_forward': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_size_t, C.c_void_p]),
+    'k4_op_distloss_backward': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_void_p, C.c_void_p,
+                                          C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    'k4_op_segment_cumsum': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    'k4_make_rays_rows':(C.c_int, [C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_int32,
                                     C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'k4_make_rays': (C.c_int, [C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_int32,
                                C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -6,7 +6,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import _lib, grid
+from . import _lib, grid, torch_efficient_distloss
 from ._scene import FusedRenderMixin, cached_host, host_float
 from .maintain import GridMaintenanceMixin
 from .coarse import CoarseStageMixin
@@ -151,3 +151,24 @@ class DirectContractedVoxGO(FusedRenderMixin, GridMaintenanceMixin, CoarseStageM
         a.d_t_list = t.data_ptr()
         a.n_t = int(t.numel())
         a.dist_thres = float((2 + 2 * self.bg_len) / self.world_len * render_kwargs['stepsize'] * 0.95)   # lib/dcvgo.py:283
+
+
+class DistortionLoss(torch.autograd.Function):
+    """lib/dcvgo.py:385-407 with the reference's signature (w, s, n_max, ray_id), on the kernels of
+    ``torch_efficient_distloss.flatten_eff_distloss``.  The forward is that loss with interval = 1 / n_max.
+
+    The backward reproduces lib/dcvgo.py:406 as written: ``grad_back * (grad_bi + grad_uni)`` with no division by
+    n = ray_id.max() + 1, so the gradient it returns is n times the gradient of its own forward (the reference's
+    quirk, kept so that a training loop that uses it behaves as it does with the reference).  Only w receives one."""
+
+    @staticmethod
+    def forward(ctx, w, s, n_max, ray_id):
+        return torch_efficient_distloss.autograd_forward(ctx, w, s, 1 / n_max, ray_id, divide_by_n=False)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_back):
+        return torch_efficient_distloss.autograd_backward(ctx, grad_back)
+
+
+distortion_loss = DistortionLoss.apply

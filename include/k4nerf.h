@@ -374,6 +374,31 @@ K4_API int k4_op_grid_sample(const float* d_grid, int32_t C, int32_t X, int32_t 
 K4_API int k4_op_grid_sample_backward(const float* d_grad_out, int32_t C, int32_t X, int32_t Y, int32_t Z, const float* h_xyz_min,
                                       const float* h_xyz_max, const float* d_xyz, int64_t M, float* d_grad_grid, k4_stream_t stream);
 
+/* The distortion loss over a flat sample list (csrc/k4_distloss.cu): d_w / d_m [n_samples] fp32, d_ray_id
+ * [n_samples] int64 non-decreasing and >= 0; a segment is a maximal run of equal ids, n = max(ray_id) + 1 (rays
+ * without samples do not count).  With the exclusive in-segment prefixes W<i, WM<i (of w and w*m) and suffixes W>i, WM>i:
+ *   L       = (sum_i 2 w_i (m_i W<i - WM<i) + interval/3 sum_i w_i^2) / n
+ *   dL/dw_i = g/n (2 m_i (W<i - W>i) + 2 (WM>i - WM<i) + 2/3 interval w_i)
+ *   torch_efficient_distloss.flatten_eff_distloss(w, m, interval, ray_id)      k4_op_distloss_forward + _backward
+ *   ub360_utils_cuda.segment_cumsum(w, s, ray_id) (the op lib/dcvgo.py:390 calls): exclusive prefixes [n_samples],
+ *       totals [n_rays] (0 for a ray without samples; ids >= n_rays are not written)   k4_op_segment_cumsum
+ * interval is d_interval[0] when d_interval != NULL (a device scalar), else the host value.  The workspace holds
+ * k4_op_distloss_workspace_bytes(n_samples) bytes, 16-byte aligned; the backward reads what the forward with the same
+ * inputs left there (n and the per-tile carries), so the forward's workspace must be kept until the backward runs.
+ * d_grad_loss is the upstream gradient g, a device scalar; divide_by_n = 0 leaves out the 1/n factor (lib/dcvgo.py:406).
+ * The loss and the gradient are bitwise reproducible (fixed summation order).  Caller's stream, no host sync.
+ * n_samples < 1, a NULL pointer or workspace: K4_ERR_INVALID_ARG; a workspace smaller than the size: K4_ERR_WORKSPACE. */
+K4_API size_t k4_op_distloss_workspace_bytes(int64_t n_samples);
+K4_API int k4_op_distloss_forward(const float* d_w, const float* d_m, const int64_t* d_ray_id, int64_t n_samples, float interval,
+                                  const float* d_interval, float* d_loss, void* d_workspace, size_t workspace_bytes,
+                                  k4_stream_t stream);
+K4_API int k4_op_distloss_backward(const float* d_w, const float* d_m, const int64_t* d_ray_id, int64_t n_samples, float interval,
+                                   const float* d_interval, const float* d_grad_loss, int32_t divide_by_n,
+                                   const void* d_workspace, size_t workspace_bytes, float* d_grad_w, k4_stream_t stream);
+K4_API int k4_op_segment_cumsum(const float* d_w, const float* d_s, const int64_t* d_ray_id, int64_t n_samples, int64_t n_rays,
+                                float* d_w_prefix, float* d_w_total, float* d_ws_prefix, float* d_ws_total, void* d_workspace,
+                                size_t workspace_bytes, k4_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Testing.  Entry points for the test suite, not for renderers: they replace no reference interface and may change
  * with the kernels they expose.
