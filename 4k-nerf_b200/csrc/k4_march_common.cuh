@@ -3,6 +3,7 @@
 // (lib/grid.py:117-128), the embeddings (lib/dvgo.py:387-388) and torch.sigmoid.
 #pragma once
 #include "k4_internal.cuh"
+#include "k4_ptx.cuh"
 
 namespace {
 
@@ -263,9 +264,7 @@ struct RgbAct {
     }
     __device__ __forceinline__ static float tc(float x, float c) {
         if constexpr (ACT == K4_ACT_GAUSS) {
-            float y;
-            asm("ex2.approx.ftz.f32 %0, %1;\n" : "=f"(y) : "f"(__fmul_rn(__fmul_rn(x, x), c)));
-            return y;
+            return ex2_approx_ftz(__fmul_rn(__fmul_rn(x, x), c));
         } else if constexpr (ACT == K4_ACT_LKRELU) {
             return x > 0.f ? x : __fmul_rn(x, 0.01f);
         } else {

@@ -11,24 +11,18 @@
 // columns), as in the blob's layout (tc_blob_layout).
 #pragma once
 #include "k4_march_common.cuh"
+#include "k4_ptx.cuh"
 #include "k4_wgmma.cuh"
-
-__device__ __forceinline__ uint32_t mlp_relu_h2(float lo, float hi) {
-    uint32_t d;
-    asm("cvt.rn.relu.satfinite.f16x2.f32 %0, %1, %2;\n" : "=r"(d) : "f"(hi), "f"(lo));
-    return d;
-}
 
 // act(lo), act(hi) as one fp16x2 word: relu stays the fused cvt.rn.relu; the other activations are evaluated in fp32
 // on the accumulator (RgbAct::tc, c = K4Dev::act_c) and rounded once.
 template <int ACT>
 __device__ __forceinline__ uint32_t mlp_act_h2(float lo, float hi, float c) {
     if constexpr (ACT == K4_ACT_RELU) {
-        return mlp_relu_h2(lo, hi);
+        return h2_relu_sat(lo, hi);
     } else {
-        uint32_t d;
-        asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;\n" : "=r"(d) : "f"(RgbAct<ACT>::tc(hi, c)), "f"(RgbAct<ACT>::tc(lo, c)));
-        return d;
+        const float h = RgbAct<ACT>::tc(hi, c), l = RgbAct<ACT>::tc(lo, c);
+        return h2_sat(l, h);
     }
 }
 
@@ -54,19 +48,14 @@ struct PhaseClock {
     static constexpr int START = K4_PHASE_SLOTS, LAST = K4_PHASE_SLOTS + 1, WORDS = K4_PHASE_SLOTS + 2;
     unsigned long long* ctr;     // [WORDS]: the counters, the group's start, the previous mark
     bool on;                     // thread 0 of the warpgroup
-    __device__ __forceinline__ static unsigned long long now() {
-        unsigned long long t;
-        asm volatile("mov.u64 %0, %%clock64;\n" : "=l"(t) :: "memory");
-        return t;
-    }
     __device__ __forceinline__ void begin() const {
         if (!on) return;
         for (int i = 0; i < K4_PHASE_SLOTS; ++i) ctr[i] = 0ull;
-        ctr[START] = ctr[LAST] = now();
+        ctr[START] = ctr[LAST] = clock64_now();
     }
     __device__ __forceinline__ void operator()(int p) const {
         if (!on) return;
-        const unsigned long long t = now();
+        const unsigned long long t = clock64_now();
         ctr[p] += t - ctr[LAST];
         ctr[LAST] = t;
     }
@@ -135,7 +124,7 @@ __device__ __forceinline__ void mlp_batch_wgmma(uint32_t a_tile, const unsigned 
     constexpr int KCH = KPAD / 8, KCHW = W / 8, NC = W / 64;      // NC: 64-column blocks of a hidden layer
     static_assert(W % 64 == 0, "hidden width");
     const int warp = wt >> 5, g = (wt & 31) >> 2, t = wt & 3;
-    const uint32_t blob_s = (uint32_t)__cvta_generic_to_shared(blob);
+    const uint32_t blob_s = smem_u32(blob);
     const uint32_t w1 = blob_s + BL.off_w1, w2 = blob_s + BL.off_w2, w3 = blob_s + BL.off_w3;
     const uint32_t b1 = blob_s + BL.off_b1, b2 = blob_s + BL.off_b2, b3 = blob_s + BL.off_b3, ones = blob_s + BL.off_ones;
     const uint64_t d_ones = wg_desc(ones, 128, 256);

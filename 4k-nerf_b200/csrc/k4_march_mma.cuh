@@ -19,6 +19,7 @@
 #pragma once
 #include "k4_internal.cuh"
 #include "k4_march_common.cuh"
+#include "k4_ptx.cuh"
 
 #ifndef K4_MARCH_THREADS
 #define K4_MARCH_THREADS 256
@@ -26,59 +27,6 @@
 #define K4_MARCH_WARPS (K4_MARCH_THREADS / 32)
 
 namespace {
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-    return (uint32_t)__cvta_generic_to_shared(p);
-}
-
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n"
-                 : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x2(uint32_t addr, uint32_t& r0, uint32_t& r1) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0,%1}, [%2];\n"
-                 : "=r"(r0), "=r"(r1) : "r"(addr));
-}
-__device__ __forceinline__ void mma16816(float c[4], const uint32_t a[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint32_t pack_h2(float lo, float hi) {
-    __half2 h = __floats2half2_rn(lo, hi);
-    return *reinterpret_cast<uint32_t*>(&h);
-}
-// hi/lo split of a pair of floats: hi = fp16(x), lo = fp16(x - hi)
-__device__ __forceinline__ void split_h2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
-    __half2 h = __floats2half2_rn(x0, x1);
-    float2 hf = __half22float2(h);
-    __half2 l = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
-    hi = *reinterpret_cast<uint32_t*>(&h);
-    lo = *reinterpret_cast<uint32_t*>(&l);
-}
-
-// ---- TMA bulk copy (global -> shared) + mbarrier, used to stage the weight pack once per CTA ----
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" :: "r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" :: "r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok = 0;
-    while (!ok) {
-        asm volatile(
-            "{\n"
-            ".reg .pred p;\n"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-            "selp.u32 %0, 1, 0, p;\n"
-            "}\n" : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    }
-}
-__device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
-                 :: "r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
 
 // Host+device description of the shared-memory weight pack (built by k4_scene.cu, one contiguous
 // blob per precision part so that a single bulk copy stages it).
@@ -178,13 +126,13 @@ struct MmaWarpCtx {
         // stage weights with one TMA bulk copy per part; biases with plain loads
         if (threadIdx.x == 0) {
             mbar_init(bar, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+            mbar_init_fence();
         }
         __syncthreads();
         if (threadIdx.x == 0) {
-            mbar_expect_tx(bar, (uint32_t)(kParts * L.part_bytes));
-            tma_bulk_g2s(w_part[0], s.wh[0], (uint32_t)L.part_bytes, bar);
-            if (kX3) tma_bulk_g2s(w_part[1], s.wl[0], (uint32_t)L.part_bytes, bar);
+            mbar_arrive_expect_tx(bar, (uint32_t)(kParts * L.part_bytes));
+            bulk_g2s(w_part[0], s.wh[0], (uint32_t)L.part_bytes, bar);
+            if (kX3) bulk_g2s(w_part[1], s.wl[0], (uint32_t)L.part_bytes, bar);
         }
         for (int i = threadIdx.x; i < L.bias_floats; i += blockDim.x) {
             int l = (i >= L.off_bias[2]) ? 2 : (i >= L.off_bias[1]) ? 1 : 0;
@@ -241,7 +189,7 @@ struct MmaWarpCtx {
                     split_h2(x[j], x[j + 1], hi, lo);
                     rh[j >> 1] = hi; rl[j >> 1] = lo;
                 } else {
-                    rh[j >> 1] = pack_h2(x[j], x[j + 1]);
+                    rh[j >> 1] = h2_rn(x[j], x[j + 1]);
                 }
             }
             qw[slot] = w;
@@ -326,18 +274,18 @@ struct MmaWarpCtx {
                                 ldsm_x4(smem_u32(w_part[0]) + off, bh[0], bh[1], bh[2], bh[3]);
 #pragma unroll
                                 for (int m = 0; m < MT; ++m) {
-                                    mma16816(acc[m][0], a1h[m][ks], bh[0], bh[1]);
-                                    mma16816(acc[m][1], a1h[m][ks], bh[2], bh[3]);
+                                    mma_16816(acc[m][0], a1h[m][ks], bh[0], bh[1]);
+                                    mma_16816(acc[m][1], a1h[m][ks], bh[2], bh[3]);
                                 }
                                 if constexpr (kX3) {
                                     uint32_t bl[4];
                                     ldsm_x4(smem_u32(w_part[1]) + off, bl[0], bl[1], bl[2], bl[3]);
 #pragma unroll
                                     for (int m = 0; m < MT; ++m) {
-                                        mma16816(acc[m][0], a1l[m][ks], bh[0], bh[1]);
-                                        mma16816(acc[m][1], a1l[m][ks], bh[2], bh[3]);
-                                        mma16816(acc[m][0], a1h[m][ks], bl[0], bl[1]);
-                                        mma16816(acc[m][1], a1h[m][ks], bl[2], bl[3]);
+                                        mma_16816(acc[m][0], a1l[m][ks], bh[0], bh[1]);
+                                        mma_16816(acc[m][1], a1l[m][ks], bh[2], bh[3]);
+                                        mma_16816(acc[m][0], a1h[m][ks], bl[0], bl[1]);
+                                        mma_16816(acc[m][1], a1h[m][ks], bl[2], bl[3]);
                                     }
                                 }
                             }
@@ -353,10 +301,10 @@ struct MmaWarpCtx {
                                 split_h2(v[4], v[5], h1h[m][np][2], h1l[m][np][2]);
                                 split_h2(v[6], v[7], h1h[m][np][3], h1l[m][np][3]);
                             } else {
-                                h1h[m][np][0] = pack_h2(v[0], v[1]);
-                                h1h[m][np][1] = pack_h2(v[2], v[3]);
-                                h1h[m][np][2] = pack_h2(v[4], v[5]);
-                                h1h[m][np][3] = pack_h2(v[6], v[7]);
+                                h1h[m][np][0] = h2_rn(v[0], v[1]);
+                                h1h[m][np][1] = h2_rn(v[2], v[3]);
+                                h1h[m][np][2] = h2_rn(v[4], v[5]);
+                                h1h[m][np][3] = h2_rn(v[6], v[7]);
                             }
                         }
                     }
@@ -388,18 +336,18 @@ struct MmaWarpCtx {
                             ldsm_x4(smem_u32(w_part[0]) + off, bh[0], bh[1], bh[2], bh[3]);
 #pragma unroll
                             for (int m = 0; m < MT; ++m) {
-                                mma16816(acc[m][0], h1h[m][ks], bh[0], bh[1]);
-                                mma16816(acc[m][1], h1h[m][ks], bh[2], bh[3]);
+                                mma_16816(acc[m][0], h1h[m][ks], bh[0], bh[1]);
+                                mma_16816(acc[m][1], h1h[m][ks], bh[2], bh[3]);
                             }
                             if constexpr (kX3) {
                                 uint32_t bl[4];
                                 ldsm_x4(smem_u32(w_part[1]) + off, bl[0], bl[1], bl[2], bl[3]);
 #pragma unroll
                                 for (int m = 0; m < MT; ++m) {
-                                    mma16816(acc[m][0], h1l[m][ks], bh[0], bh[1]);
-                                    mma16816(acc[m][1], h1l[m][ks], bh[2], bh[3]);
-                                    mma16816(acc[m][0], h1h[m][ks], bl[0], bl[1]);
-                                    mma16816(acc[m][1], h1h[m][ks], bl[2], bl[3]);
+                                    mma_16816(acc[m][0], h1l[m][ks], bh[0], bh[1]);
+                                    mma_16816(acc[m][1], h1l[m][ks], bh[2], bh[3]);
+                                    mma_16816(acc[m][0], h1h[m][ks], bl[0], bl[1]);
+                                    mma_16816(acc[m][1], h1h[m][ks], bl[2], bl[3]);
                                 }
                             }
                         }
@@ -419,13 +367,13 @@ struct MmaWarpCtx {
                             split_h2(v[0], v[1], ah[0], al[0]); split_h2(v[2], v[3], ah[1], al[1]);
                             split_h2(v[4], v[5], ah[2], al[2]); split_h2(v[6], v[7], ah[3], al[3]);
                         } else {
-                            ah[0] = pack_h2(v[0], v[1]); ah[1] = pack_h2(v[2], v[3]);
-                            ah[2] = pack_h2(v[4], v[5]); ah[3] = pack_h2(v[6], v[7]);
+                            ah[0] = h2_rn(v[0], v[1]); ah[1] = h2_rn(v[2], v[3]);
+                            ah[2] = h2_rn(v[4], v[5]); ah[3] = h2_rn(v[6], v[7]);
                         }
-                        mma16816(acc3[m], ah, b3h[0], b3h[1]);
+                        mma_16816(acc3[m], ah, b3h[0], b3h[1]);
                         if constexpr (kX3) {
-                            mma16816(acc3[m], al, b3h[0], b3h[1]);
-                            mma16816(acc3[m], ah, b3l[0], b3l[1]);
+                            mma_16816(acc3[m], al, b3h[0], b3h[1]);
+                            mma_16816(acc3[m], ah, b3l[0], b3l[1]);
                         }
                     }
                 }

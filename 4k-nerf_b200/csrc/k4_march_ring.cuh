@@ -1,63 +1,24 @@
 // k4_march_ring.cuh -- what the two wgmma marchers (k4_march_tc.cu, k4_march_ws.cu) share beyond k4_march_ray.cuh:
-// the PTX helpers, the config (derived constants and shared-memory map), the TMA staging of the operand blob, the packed
-// view embedding of a ray and the features of a surviving sample.  Each kernel reserves ring rows and stores them itself:
+// the config (derived constants and shared-memory map), the TMA staging of the operand blob, the packed view embedding
+// of a ray and the features of a surviving sample.  Each kernel reserves ring rows and stores them itself:
 // k4_march_ws.cu packs a row chunk by chunk with the view words read from shared memory to stay under its 128 registers,
-// k4_march_tc.cu builds the row in registers.
+// k4_march_tc.cu builds the row in registers.  Marcher group wg synchronises its warpgroup on named barrier wg + 1.
 #pragma once
 #include "k4_internal.cuh"
 #include "k4_march_common.cuh"
 #include "k4_march_mlp.cuh"
+#include "k4_ptx.cuh"
 
 namespace {
 
 constexpr int TC_WG = 128;           // threads of a warpgroup = rays of a tile = rows of an MLP batch
 constexpr int TC_ROUND = 8;          // marching steps between warpgroup rendezvous when nothing is pending
 
-// ---------------------------------------------------------------------------------------------
-// PTX helpers
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" :: "r"(s_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok = 0;
-    while (!ok) {
-        asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n"
-                     : "=r"(ok) : "r"(s_u32(bar)), "r"(parity) : "memory");
-    }
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" :: "r"(s_u32(bar)) : "memory");
-}
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile("{\n.reg .pred p;\nmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n"
-                 : "=r"(ok) : "r"(s_u32(bar)), "r"(parity) : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ uint32_t pack2(float lo, float hi) {
-    uint32_t d;      // saturating: a feature beyond the fp16 range becomes +-65504, never inf
-    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;\n" : "=r"(d) : "f"(hi), "f"(lo));
-    return d;
-}
-// named barrier `id` over the 128 threads of a warpgroup (marcher group wg uses id wg + 1; 0 is __syncthreads), and its
-// form that also ORs a predicate over them
-__device__ __forceinline__ void named_bar(int id) { asm volatile("bar.sync %0, 128;\n" :: "r"(id) : "memory"); }
-__device__ __forceinline__ bool named_bar_or(int id, bool pred) {
-    uint32_t r;
-    asm volatile("{\n.reg .pred p, q;\nsetp.ne.u32 p, %2, 0;\nbarrier.cta.red.or.pred q, %1, 128, p;\nselp.u32 %0, 1, 0, q;\n}\n"
-                 : "=r"(r) : "r"(id), "r"((uint32_t)pred) : "memory");
-    return r != 0;
-}
-
 // The operand blob (weights + bias tiles) from global to shared memory as one TMA bulk copy that completes on `bar`.
 // One thread calls it, once bar's mbarrier.init is visible; everybody then waits for phase 0 of bar.
 __device__ __forceinline__ void stage_blob(unsigned char* blob, const void* src, int bytes, uint64_t* bar) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" :: "r"(s_u32(bar)), "r"((uint32_t)bytes) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
-                 :: "r"(s_u32(blob)), "l"(src), "r"((uint32_t)bytes), "r"(s_u32(bar)) : "memory");
+    mbar_arrive_expect_tx(bar, (uint32_t)bytes);
+    bulk_g2s(blob, src, (uint32_t)bytes, bar);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -122,7 +83,7 @@ __device__ __forceinline__ void pack_view_embedding(Vec3 v, uint32_t vw[Cfg::NVW
         }
     ve[Cfg::NVEMB] = 0.f;
 #pragma unroll
-    for (int j = 0; j < Cfg::NVW; ++j) vw[j] = pack2(ve[2 * j], ve[2 * j + 1]);
+    for (int j = 0; j < Cfg::NVW; ++j) vw[j] = h2_sat(ve[2 * j], ve[2 * j + 1]);
 }
 
 // ---------------------------------------------------------------------------------------------

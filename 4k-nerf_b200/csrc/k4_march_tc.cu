@@ -48,7 +48,7 @@ k4_march_tc_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
     // ---------------- one-time CTA setup ----------------
     if (tid == 0) {
         mbar_init(wbar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+        mbar_init_fence();
     }
     {   // zero this warpgroup's block (A rings incl. their K padding, accumulators, counters)
         uint32_t* z = reinterpret_cast<uint32_t*>(wgb);
@@ -57,7 +57,7 @@ k4_march_tc_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
     __syncthreads();
     if (tid == 0) stage_blob(blob, s.tc_blob, BL.total, wbar);
     mbar_wait(wbar, 0);
-    const uint32_t a_ring_s = s_u32(wgb);
+    const uint32_t a_ring_s = smem_u32(wgb);
 
     unsigned head = 0;
     unsigned long long tot_m = 0, tot_d = 0, tot_c = 0, n_batches = 0;
@@ -66,7 +66,7 @@ k4_march_tc_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
     // One MLP batch over ring rows [head, head+128); `valid` of them are real samples.
     auto flush = [&](int valid) {
         const uint32_t a_tile = a_ring_s + ((head >> 7) & 1u) * Cfg::TILE_BYTES;
-        asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");      // generic smem writes -> async proxy
+        fence_proxy_async();
         named_bar(wg + 1);
         if (wt == 0) ++n_batches;
         mlp_batch_wgmma<W, KPAD, true, ACT>(a_tile, blob, BL, valid, head & (TC_RING - 1), qw, qowner, nullptr, racc, wt, s.act_c,
@@ -139,7 +139,7 @@ k4_march_tc_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
                         uint32_t row[KPAD / 2];
 #pragma unroll
                         for (int j = 0; j < KPAD / 2; ++j) {
-                            if (j < Cfg::NS / 2) row[j] = pack2(f[2 * j], f[2 * j + 1]);
+                            if (j < Cfg::NS / 2) row[j] = h2_sat(f[2 * j], f[2 * j + 1]);
                             else if (j < Cfg::NS / 2 + Cfg::NVW) row[j] = vw[j - Cfg::NS / 2];
                             else row[j] = 0u;
                         }

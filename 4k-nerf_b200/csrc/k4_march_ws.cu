@@ -70,7 +70,7 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
             mbar_init(&wg_ctl(g)->full_bar, 1);
             mbar_init(&wg_ctl(g)->done_bar, 128);
         }
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+        mbar_init_fence();
     }
     __syncthreads();
     if (tid == 0) stage_blob(blob, s.tc_blob, BL.total, wbar);
@@ -85,7 +85,7 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
         // =====================================================================================
         const int g = wg - 2;
         WgCtl* c = wg_ctl(g);
-        const uint32_t ring_s = s_u32(wg_base(g));
+        const uint32_t ring_s = smem_u32(wg_base(g));
         const float* qw = reinterpret_cast<const float*>(wg_base(g) + Cfg::WG_QW);
         const unsigned char* qowner = wg_base(g) + Cfg::WG_OWNER;
         const float* qdiff = reinterpret_cast<const float*>(wg_base(g) + Cfg::WG_QDIFF);
@@ -142,7 +142,7 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
         // colours are in racc (other batches arrive as soon as their rows are read, before their epilogue).
         bool tile_open = false;            // a batch of this ray tile was submitted without `last`
         auto submit = [&](int valid, bool last) {
-            asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");      // generic smem writes -> async proxy
+            fence_proxy_async();
             named_bar(wg + 1);
             mark(K4_PH_M_RENDEZVOUS);
             while (n_done < n_sub) { mbar_wait(&ctl->done_bar, done_ph); done_ph ^= 1; ++n_done; }
@@ -232,7 +232,7 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
 #pragma unroll
                                 for (int e = 0; e < 4; ++e) {
                                     const int j = 4 * kc + e;
-                                    if (j < Cfg::NS / 2) q[e] = pack2(f[Cfg::K0OFF + 2 * j], f[Cfg::K0OFF + 2 * j + 1]);
+                                    if (j < Cfg::NS / 2) q[e] = h2_sat(f[Cfg::K0OFF + 2 * j], f[Cfg::K0OFF + 2 * j + 1]);
                                     else if (j < Cfg::NS / 2 + Cfg::NVW) q[e] = vws[(j - Cfg::NS / 2) * 128];
                                     else q[e] = 0u;
                                 }
@@ -308,7 +308,7 @@ int launch_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st, unsigned l
 }
 
 // k4_testing_rgbnet, wgmma modes: one CTA = one warpgroup = one batch of up to 128 caller rows.  The operand blob is staged
-// as the marchers stage it; row r goes to ring-tile row r through the scene's column map (pack2, other columns zero), its
+// as the marchers stage it; row r goes to ring-tile row r through the scene's column map (h2_sat, other columns zero), its
 // weight / owner / diffuse logits to the queue, and mlp_batch_wgmma accumulates the colours into racc.
 template <class Cfg, int ACT>
 __global__ void __launch_bounds__(TC_WG, 1)
@@ -328,7 +328,7 @@ k4_test_rgbnet_ws_kernel(const __grid_constant__ K4Dev s, const float* __restric
 
     if (wt == 0) {
         mbar_init(bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+        mbar_init_fence();
     }
     __syncthreads();
     if (wt == 0) stage_blob(blob, s.tc_blob, BL.total, bar);
@@ -343,8 +343,8 @@ k4_test_rgbnet_ws_kernel(const __grid_constant__ K4Dev s, const float* __restric
     unsigned char* rowp = tile + tc_canon_off(wt, 0, KCH);
 #pragma unroll
     for (int kc = 0; kc < KCH; ++kc)
-        *reinterpret_cast<uint4*>(rowp + kc * 128) = make_uint4(pack2(f[8 * kc + 0], f[8 * kc + 1]), pack2(f[8 * kc + 2], f[8 * kc + 3]),
-                                                                pack2(f[8 * kc + 4], f[8 * kc + 5]), pack2(f[8 * kc + 6], f[8 * kc + 7]));
+        *reinterpret_cast<uint4*>(rowp + kc * 128) = make_uint4(h2_sat(f[8 * kc + 0], f[8 * kc + 1]), h2_sat(f[8 * kc + 2], f[8 * kc + 3]),
+                                                                h2_sat(f[8 * kc + 4], f[8 * kc + 5]), h2_sat(f[8 * kc + 6], f[8 * kc + 7]));
     qw[wt] = wt < valid ? ws[r] : 0.f;
     qowner[wt] = (unsigned char)(wt < valid ? (owners[r] & (TC_WG - 1)) : 0);
 #pragma unroll
@@ -352,10 +352,10 @@ k4_test_rgbnet_ws_kernel(const __grid_constant__ K4Dev s, const float* __restric
         qdiff[3 * wt + c] = (diffs && wt < valid) ? diffs[3 * r + c] : 0.f;
         racc[3 * wt + c] = 0.f;
     }
-    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");      // generic smem writes -> async proxy
+    fence_proxy_async();
     mbar_wait(bar, 0);
     __syncthreads();
-    mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0, ACT>(s_u32(tile), blob, BL, valid, 0u, qw, qowner, qdiff, racc, wt, s.act_c, [] {}, true);
+    mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0, ACT>(smem_u32(tile), blob, BL, valid, 0u, qw, qowner, qdiff, racc, wt, s.act_c, [] {}, true);
     __syncthreads();
 #pragma unroll
     for (int c = 0; c < 3; ++c) racc_out[3 * (r0 + wt) + c] = racc[3 * wt + c];

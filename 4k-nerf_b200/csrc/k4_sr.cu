@@ -24,34 +24,17 @@
 #include <new>
 
 #include "k4_internal.cuh"
+#include "k4_ptx.cuh"
 #include "k4_wgmma.cuh"
 
-namespace {
+// Intermediate activations and the condition map are rounded to fp16 with h2_sat: those of a trained checkpoint may
+// exceed the fp16 range, and a clamped operand degrades gracefully where an inf poisons the frame.
+//
+// Programmatic dependent launch: every decoder kernel is launched with programmaticStreamSerialization (sr_launch), so
+// its CTAs are scheduled while the previous kernel drains; what a kernel does before its pdl_wait_and_release()
+// (barrier init, constant weights) overlaps the predecessor's tail.
 
-// ---------------------------------------------------------------------------------------------
-// plumbing
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t sr_s32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void sr_mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" :: "r"(sr_s32(bar)), "r"(count));
-}
-__device__ __forceinline__ void sr_mbar_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok = 0;
-    while (!ok) {
-        asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n"
-                     : "=r"(ok) : "r"(sr_s32(bar)), "r"(parity) : "memory");
-    }
-}
-// fp32 pair -> fp16x2, round to nearest, SATURATING (|x| > 65504 -> +-65504 instead of inf): activations of a
-// trained checkpoint may exceed the fp16 range; a clamped operand degrades gracefully, an inf poisons the frame.
-__device__ __forceinline__ __half2 sr_h2sat(float lo, float hi) {
-    uint32_t d;
-    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;\n" : "=r"(d) : "f"(hi), "f"(lo));
-    return *reinterpret_cast<__half2*>(&d);
-}
-__device__ __forceinline__ void cp_async16(void* dst_smem, const void* src, int src_bytes) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" :: "r"(sr_s32(dst_smem)), "l"(src), "r"(src_bytes) : "memory");
-}
+namespace {
 
 constexpr int SR_TY = 16;                            // output rows of a tile
 constexpr int SR_HY = SR_TY + 2;                     // halo rows
@@ -120,16 +103,6 @@ __host__ __device__ inline SftFrag sft_frag_layout(int n) {
 }
 constexpr int SFTF_MAX = 2 * (3 * 64 * SFTF_PITCH * 2 + 3 * 64 * 4);      // two 64-channel layers: 32,256 B
 
-__device__ __forceinline__ void sr_hmma(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint32_t sr_pack_sat(float lo, float hi) {
-    uint32_t d;
-    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;\n" : "=r"(d) : "f"(hi), "f"(lo));
-    return d;
-}
-
 // Hidden layer of one SFT layer for 16 pixels: cond fragments `ca` (m16 x k32) x W0 (64 outputs) -> LeakyReLU -> the A
 // fragments of the two second GEMMs (scale branch: hidden 0..31, shift branch: hidden 32..63).  The accumulator fragment
 // of two adjacent n8 blocks IS the A fragment of one k16 step (rows g / g+8, columns 2t..2t+1 / +8).
@@ -144,14 +117,14 @@ __device__ __forceinline__ void sft_hidden(const unsigned char* fw, const SftFra
 #pragma unroll
         for (int ks = 0; ks < 2; ++ks) {
             const __half* wr = W0 + (8 * j + g) * SFTF_PITCH + 16 * ks + 2 * tq;
-            sr_hmma(c, ca[ks], *reinterpret_cast<const uint32_t*>(wr), *reinterpret_cast<const uint32_t*>(wr + 8));
+            mma_16816(c, ca[ks], *reinterpret_cast<const uint32_t*>(wr), *reinterpret_cast<const uint32_t*>(wr + 8));
         }
 #pragma unroll
         for (int e = 0; e < 4; ++e) c[e] = fmaxf(c[e], 0.2f * c[e]);
         uint32_t (&dst)[2][4] = (j < 4) ? as : ah;
         const int jj = j & 3;
-        dst[jj >> 1][(jj & 1) * 2 + 0] = sr_pack_sat(c[0], c[1]);          // row g
-        dst[jj >> 1][(jj & 1) * 2 + 1] = sr_pack_sat(c[2], c[3]);          // row g + 8
+        dst[jj >> 1][(jj & 1) * 2 + 0] = h2_sat(c[0], c[1]);          // row g
+        dst[jj >> 1][(jj & 1) * 2 + 1] = h2_sat(c[2], c[3]);          // row g + 8
     }
 }
 // scale + 1 and shift of output channels 8j .. 8j+7 for the 16 pixels (accumulator fragment layout)
@@ -167,17 +140,10 @@ __device__ __forceinline__ void sft_scale_shift(const unsigned char* fw, const S
     for (int ks = 0; ks < 2; ++ks) {
         const __half* ws = W1s + (8 * j + g) * SFTF_PITCH + 16 * ks + 2 * tq;
         const __half* wh = W1h + (8 * j + g) * SFTF_PITCH + 16 * ks + 2 * tq;
-        sr_hmma(sc, as[ks], *reinterpret_cast<const uint32_t*>(ws), *reinterpret_cast<const uint32_t*>(ws + 8));
-        sr_hmma(sh, ah[ks], *reinterpret_cast<const uint32_t*>(wh), *reinterpret_cast<const uint32_t*>(wh + 8));
+        mma_16816(sc, as[ks], *reinterpret_cast<const uint32_t*>(ws), *reinterpret_cast<const uint32_t*>(ws + 8));
+        mma_16816(sh, ah[ks], *reinterpret_cast<const uint32_t*>(wh), *reinterpret_cast<const uint32_t*>(wh + 8));
     }
 }
-// Programmatic dependent launch: every decoder kernel is launched with programmaticStreamSerialization, so its CTAs are
-// scheduled while the previous kernel drains; the set-up above this point (barrier init, constant
-// weights) overlaps the predecessor's tail.  Nothing produced by an earlier kernel may be touched before the wait; the
-// dependents are released only after it, so at most two consecutive kernels are ever in flight.
-#define SR_PDL_SYNC() do { asm volatile("griddepcontrol.wait;\n" ::: "memory"); \
-                           asm volatile("griddepcontrol.launch_dependents;\n" ::: "memory"); } while (0)
-
 // ---------------------------------------------------------------------------------------------
 // conv3x3_ws_kernel<N>: every 3x3 convolution as an im2col-free implicit GEMM on Hopper warpgroup MMAs --
 // ONE persistent CTA per SM, warp specialised, fed through a deep shared-memory ring:
@@ -214,10 +180,6 @@ template <int N> struct WsCfg {
     static constexpr int NST = (N >= 64) ? 5 : 6;
     static constexpr int SMEM = NST * STAGE + 512;              // + barriers (256 B) + bias (256 B)
 };
-
-__device__ __forceinline__ void ws_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" :: "r"(sr_s32(bar)) : "memory");
-}
 
 // ---------------------------------------------------------------------------------------------
 // Epilogue of one 16-pixel block with the following SFT layer(s) folded in (SRM_*_SFT* modes).  The 36 SFT layers of the
@@ -287,8 +249,8 @@ __device__ __forceinline__ void epilogue_sft(const ConvParams& p, const unsigned
         if (!trunk) {                       // SRM_STORE_F16_SFT
 #pragma unroll
             for (int e = 0; e < 4; ++e) { const float a = p.lrelu > 0.f ? fmaxf(v[e], p.lrelu * v[e]) : v[e]; v[e] = fmaf(a, sc[e], sh[e]); }
-            if (inA) *reinterpret_cast<uint32_t*>(p.dst_h + pixA * p.dst_cstride + p.dst_c0 + ch) = sr_pack_sat(v[0], v[1]);
-            if (inB) *reinterpret_cast<uint32_t*>(p.dst_h + pixB * p.dst_cstride + p.dst_c0 + ch) = sr_pack_sat(v[2], v[3]);
+            if (inA) *reinterpret_cast<uint32_t*>(p.dst_h + pixA * p.dst_cstride + p.dst_c0 + ch) = h2_sat(v[0], v[1]);
+            if (inB) *reinterpret_cast<uint32_t*>(p.dst_h + pixB * p.dst_cstride + p.dst_c0 + ch) = h2_sat(v[2], v[3]);
             continue;
         }
         float t[4] = {fmaf(v[0], p.scale, rA[sl].x), fmaf(v[1], p.scale, rA[sl].y), fmaf(v[2], p.scale, rB[sl].x), fmaf(v[3], p.scale, rB[sl].y)};
@@ -314,8 +276,8 @@ __device__ __forceinline__ void epilogue_sft(const ConvParams& p, const unsigned
 #pragma unroll
             for (int e = 0; e < 4; ++e) t[e] = fmaf(t[e], sc[e], sh[e]);
         }
-        if (inA) *reinterpret_cast<uint32_t*>(p.dst_h2 + pixA * p.dst2_cstride + p.dst2_c0 + ch) = sr_pack_sat(t[0], t[1]);
-        if (inB) *reinterpret_cast<uint32_t*>(p.dst_h2 + pixB * p.dst2_cstride + p.dst2_c0 + ch) = sr_pack_sat(t[2], t[3]);
+        if (inA) *reinterpret_cast<uint32_t*>(p.dst_h2 + pixA * p.dst2_cstride + p.dst2_c0 + ch) = h2_sat(t[0], t[1]);
+        if (inB) *reinterpret_cast<uint32_t*>(p.dst_h2 + pixB * p.dst2_cstride + p.dst2_c0 + ch) = h2_sat(t[2], t[3]);
     }
 }
 
@@ -336,13 +298,13 @@ __device__ __forceinline__ void epilogue_plain(const ConvParams& p, const float*
             float o0 = acc[4 * j + 2 * r] + sbias[ch], o1 = acc[4 * j + 2 * r + 1] + sbias[ch + 1];
             if (p.mode == SRM_STORE_F16) {
                 if (p.lrelu > 0.f) { o0 = o0 > 0.f ? o0 : o0 * p.lrelu; o1 = o1 > 0.f ? o1 : o1 * p.lrelu; }
-                *reinterpret_cast<uint32_t*>(p.dst_h + pix * p.dst_cstride + p.dst_c0 + ch) = sr_pack_sat(o0, o1);
+                *reinterpret_cast<uint32_t*>(p.dst_h + pix * p.dst_cstride + p.dst_c0 + ch) = h2_sat(o0, o1);
             } else if (p.mode == SRM_TRUNK) {
                 const float2 a = __ldg(reinterpret_cast<const float2*>(p.add_f + pix * 64 + ch));
                 *reinterpret_cast<float2*>(p.dst_f + pix * 64 + ch) = make_float2(o0 * p.scale + a.x, o1 * p.scale + a.y);
             } else if (p.mode == SRM_ADD_STORE_F16) {
                 const float2 a = __ldg(reinterpret_cast<const float2*>(p.add_f + pix * 64 + ch));
-                *reinterpret_cast<uint32_t*>(p.dst_h + pix * p.dst_cstride + p.dst_c0 + ch) = sr_pack_sat(o0 + a.x, o1 + a.y);
+                *reinterpret_cast<uint32_t*>(p.dst_h + pix * p.dst_cstride + p.dst_c0 + ch) = h2_sat(o0 + a.x, o1 + a.y);
             } else if (p.mode == SRM_STORE_F32F16) {
                 *reinterpret_cast<float2*>(p.dst_f + pix * 64 + ch) = make_float2(o0, o1);
                 if (p.dst_f2) *reinterpret_cast<float2*>(p.dst_f2 + pix * 64 + ch) = make_float2(o0, o1);
@@ -378,14 +340,14 @@ __global__ void __launch_bounds__(WS_THREADS, 1) conv3x3_ws_kernel(const __grid_
     const int nchunks = p.cin / SR_CK;
 
     if (tid == 0) {
-        for (int i = 0; i < C::NST; ++i) { sr_mbar_init(full + i, p.use_tma ? 1 : 128); sr_mbar_init(empty + i, 8); }
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+        for (int i = 0; i < C::NST; ++i) { mbar_init(full + i, p.use_tma ? 1 : 128); mbar_init(empty + i, 8); }
+        mbar_init_fence();
     }
     __syncthreads();
-    SR_PDL_SYNC();
+    pdl_wait_and_release();
 
     if (wg == 2) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 56;\n");
+        setmaxnreg_dec<56>();
         if (p.use_tma) {
             // ------------------------------ producer (TMA): one thread, three bulk copies per stage ------------------------------
             // The activation buffer is a 3-D tensor (channel, x, y); a box of (8 channels, 34, 18) lands in shared
@@ -398,17 +360,14 @@ __global__ void __launch_bounds__(WS_THREADS, 1) conv3x3_ws_kernel(const __grid_
                     const int y0 = p.y_lo + ty * SR_TY - 1, x0 = tx * WS_TX - 1;
                     for (int c = 0; c < nchunks; ++c, ++g) {
                         const unsigned slot = g % C::NST;
-                        if (g >= (unsigned)C::NST) sr_mbar_wait(empty + slot, ((g / C::NST) - 1) & 1);
-                        const uint32_t bar = sr_s32(full + slot);
-                        const uint32_t A = sr_s32(smem + slot * C::STAGE);
+                        if (g >= (unsigned)C::NST) mbar_wait(empty + slot, ((g / C::NST) - 1) & 1);
+                        uint64_t* bar = full + slot;
+                        unsigned char* A = smem + slot * C::STAGE;
                         const uint32_t bbytes = (uint32_t)p.ntaps * C::B_TAP;
-                        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" :: "r"(bar), "r"((uint32_t)((SR_CK / 8) * SR_HY * WS_ROW) + bbytes) : "memory");
+                        mbar_arrive_expect_tx(bar, (uint32_t)((SR_CK / 8) * SR_HY * WS_ROW) + bbytes);
 #pragma unroll
-                        for (int pl = 0; pl < SR_CK / 8; ++pl)
-                            asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];\n"
-                                         :: "r"(A + pl * WS_PLANE), "l"(tm), "r"(bar), "r"(c * SR_CK + pl * 8), "r"(x0), "r"(y0) : "memory");
-                        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
-                                     :: "r"(A + WS_A_STAGE), "l"(p.wpack + (size_t)c * bbytes), "r"(bbytes), "r"(bar) : "memory");
+                        for (int pl = 0; pl < SR_CK / 8; ++pl) tensor_g2s_3d(A + pl * WS_PLANE, tm, bar, c * SR_CK + pl * 8, x0, y0);
+                        bulk_g2s(A + WS_A_STAGE, p.wpack + (size_t)c * bbytes, bbytes, bar);
                     }
                 }
             }
@@ -418,15 +377,15 @@ __global__ void __launch_bounds__(WS_THREADS, 1) conv3x3_ws_kernel(const __grid_
             const int sW = p.upsample ? (p.W >> 1) : p.W;
             unsigned g = 0;
             auto publish = [&](unsigned gi) {
-                asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-                ws_arrive(full + gi % C::NST);
+                fence_proxy_async();
+                mbar_arrive(full + gi % C::NST);
             };
             for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
                 const int ty = tile / tiles_x, tx = tile - ty * tiles_x;
                 const int y0 = p.y_lo + ty * SR_TY, x0 = tx * WS_TX;
                 for (int c = 0; c < nchunks; ++c, ++g) {
                     const unsigned slot = g % C::NST;
-                    if (g >= (unsigned)C::NST) sr_mbar_wait(empty + slot, ((g / C::NST) - 1) & 1);
+                    if (g >= (unsigned)C::NST) mbar_wait(empty + slot, ((g / C::NST) - 1) & 1);
                     unsigned char* A = smem + slot * C::STAGE;
 #pragma unroll 1
                     for (int j = 0; j < WS_HALO_PER_THREAD; ++j) {
@@ -445,22 +404,22 @@ __global__ void __launch_bounds__(WS_THREADS, 1) conv3x3_ws_kernel(const __grid_
                     const unsigned char* wsrc = p.wpack + (size_t)c * bbytes;
                     unsigned char* B = A + WS_A_STAGE;
                     for (int i = pt; i < bbytes / 16; i += 128) cp_async16(B + i * 16, wsrc + i * 16, 16);
-                    asm volatile("cp.async.commit_group;\n" ::: "memory");
+                    cp_async_commit();
                     if (g >= (unsigned)WS_LAG) {
-                        asm volatile("cp.async.wait_group %0;\n" :: "n"(WS_LAG) : "memory");
+                        cp_async_wait<WS_LAG>();
                         publish(g - WS_LAG);
                     }
                 }
             }
             // drain: the last WS_LAG stages
-            if (g >= 2) { asm volatile("cp.async.wait_group 1;\n" ::: "memory"); publish(g - 2); }
-            if (g >= 1) { asm volatile("cp.async.wait_group 0;\n" ::: "memory"); publish(g - 1); }
+            if (g >= 2) { cp_async_wait<1>(); publish(g - 2); }
+            if (g >= 1) { cp_async_wait<0>(); publish(g - 1); }
         }
     } else {
         // ------------------------------ consumers: MMAs + epilogue of M tiles 2*wg, 2*wg+1 ------------------------------
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 224;\n");
+        setmaxnreg_inc<224>();
         const int lane = tid & 31, wq = warp & 3, g8 = lane >> 2, tq = lane & 3;
-        const uint32_t smem_s = sr_s32(smem);
+        const uint32_t smem_s = smem_u32(smem);
         unsigned g = 0;
         for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
             const int ty = tile / tiles_x, tx = tile - ty * tiles_x;
@@ -468,7 +427,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) conv3x3_ws_kernel(const __grid_
             float acc[2][2][N / 2];                                  // [M tile of this group][m64 half][fragment]
             for (int c = 0; c < nchunks; ++c, ++g) {
                 const unsigned slot = g % C::NST;
-                sr_mbar_wait(full + slot, (g / C::NST) & 1);
+                mbar_wait(full + slot, (g / C::NST) & 1);
                 const uint32_t a0 = smem_s + slot * C::STAGE, b0 = a0 + WS_A_STAGE;
                 wg_fence();
 #pragma unroll
@@ -487,10 +446,10 @@ __global__ void __launch_bounds__(WS_THREADS, 1) conv3x3_ws_kernel(const __grid_
                 wg_commit();
                 // the previous stage's MMAs have retired once at most this stage's group is pending
                 wg_wait<1>();
-                if (c > 0 && lane == 0) ws_arrive(empty + (g - 1) % C::NST);
+                if (c > 0 && lane == 0) mbar_arrive(empty + (g - 1) % C::NST);
             }
             wg_wait<0>();
-            if (lane == 0) ws_arrive(empty + (g - 1) % C::NST);
+            if (lane == 0) mbar_arrive(empty + (g - 1) % C::NST);
 #pragma unroll
             for (int ml = 0; ml < 2; ++ml)
 #pragma unroll
@@ -557,9 +516,9 @@ __global__ void __launch_bounds__(K64_THREADS, 1) conv3x3_k64_kernel(const __gri
     const int n_tiles = tiles_x * tiles_y;
 
     if (tid == 0) {
-        for (int i = 0; i < C::NST; ++i) { sr_mbar_init(full + i, 1); sr_mbar_init(empty + i, 8); }
-        sr_mbar_init(wbar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+        for (int i = 0; i < C::NST; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, 8); }
+        mbar_init(wbar, 1);
+        mbar_init_fence();
     }
     __syncthreads();
 
@@ -567,35 +526,31 @@ __global__ void __launch_bounds__(K64_THREADS, 1) conv3x3_k64_kernel(const __gri
         // ------------------------------ producer: weights once, then one tensor copy per tile ------------------------------
         if (tid == 256) {
             const uint64_t ta = reinterpret_cast<uint64_t>(&tmap_a), tb = reinterpret_cast<uint64_t>(&tmap_b);
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" :: "r"(sr_s32(wbar)), "r"((uint32_t)p.ntaps * C::B_TAP) : "memory");
-            for (int t = 0; t < p.ntaps; ++t)
-                asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];\n"
-                             :: "r"(sr_s32(Bw + t * C::B_TAP)), "l"(tb), "r"(sr_s32(wbar)), "r"(0), "r"(t * N) : "memory");
-            SR_PDL_SYNC();                                        // the weights above are constants; the activations are not
+            mbar_arrive_expect_tx(wbar, (uint32_t)p.ntaps * C::B_TAP);
+            for (int t = 0; t < p.ntaps; ++t) tensor_g2s_2d(Bw + t * C::B_TAP, tb, wbar, 0, t * N);
+            pdl_wait_and_release();                               // the weights above are constants; the activations are not
             unsigned g = 0;
             for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++g) {
                 const int ty = tile / tiles_x, tx = tile - ty * tiles_x;
                 const unsigned slot = g % C::NST;
-                if (g >= (unsigned)C::NST) sr_mbar_wait(empty + slot, ((g / C::NST) - 1) & 1);
-                const uint32_t bar = sr_s32(full + slot);
-                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" :: "r"(bar), "r"((uint32_t)K64_A_BYTES) : "memory");
-                asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];\n"
-                             :: "r"(sr_s32(Ar + slot * K64_A_STAGE)), "l"(ta), "r"(bar), "r"(0), "r"(tx * K64_TX - 1), "r"(p.y_lo + ty * SR_TY - 1) : "memory");
+                if (g >= (unsigned)C::NST) mbar_wait(empty + slot, ((g / C::NST) - 1) & 1);
+                mbar_arrive_expect_tx(full + slot, (uint32_t)K64_A_BYTES);
+                tensor_g2s_3d(Ar + slot * K64_A_STAGE, ta, full + slot, 0, tx * K64_TX - 1, p.y_lo + ty * SR_TY - 1);
             }
         }
     } else {
         // ------------------------------ consumers: m64 halves 3*wg .. 3*wg+2 (M tile j/2, image rows 8*(j%2) ..) ------------------------------
-        SR_PDL_SYNC();                                            // residual reads / output writes touch earlier kernels' buffers
+        pdl_wait_and_release();                                   // residual reads / output writes touch earlier kernels' buffers
         const int lane = tid & 31, wq = warp & 3, g8 = lane >> 2, tq = lane & 3;
-        sr_mbar_wait(wbar, 0);
-        const uint32_t bw = sr_s32(Bw);
+        mbar_wait(wbar, 0);
+        const uint32_t bw = smem_u32(Bw);
         unsigned g = 0;
         for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++g) {
             const int ty = tile / tiles_x, tx = tile - ty * tiles_x;
             const int y0 = p.y_lo + ty * SR_TY, x0 = tx * K64_TX;
             const unsigned slot = g % C::NST;
-            sr_mbar_wait(full + slot, (g / C::NST) & 1);
-            const uint32_t a0 = sr_s32(Ar + slot * K64_A_STAGE);
+            mbar_wait(full + slot, (g / C::NST) & 1);
+            const uint32_t a0 = smem_u32(Ar + slot * K64_A_STAGE);
             float acc[3][N / 2];
             wg_fence();
 #pragma unroll
@@ -616,7 +571,7 @@ __global__ void __launch_bounds__(K64_THREADS, 1) conv3x3_k64_kernel(const __gri
             }
             wg_commit();
             wg_wait<0>();
-            if (lane == 0) ws_arrive(empty + slot);
+            if (lane == 0) mbar_arrive(empty + slot);
 #pragma unroll
             for (int h = 0; h < 3; ++h) {
                 wg_fence_acc(acc[h]);
@@ -683,9 +638,9 @@ __global__ void __launch_bounds__(128) sft_kernel(const __grid_constant__ SftPar
 #pragma unroll
             for (int j = 0; j < 8; ++j) p.dst_f[pix * 64 + o0 + j] = y[j] * p.res_scale + __ldg(p.res_f + pix * 64 + o0 + j);
         } else {
-            __half2 h[4];
+            uint32_t h[4];
 #pragma unroll
-            for (int j = 0; j < 4; ++j) h[j] = sr_h2sat(y[2 * j], y[2 * j + 1]);
+            for (int j = 0; j < 4; ++j) h[j] = h2_sat(y[2 * j], y[2 * j + 1]);
             *reinterpret_cast<uint4*>(p.dst_h + pix * p.dst_cstride + p.dst_c0 + o0) = *reinterpret_cast<uint4*>(h);
         }
     }
@@ -703,7 +658,7 @@ __global__ void __launch_bounds__(128) sft_mma_kernel(const __grid_constant__ Sf
     const SftFrag L = sft_frag_layout(COUT);
     for (int i = threadIdx.x; i < L.total / 16; i += blockDim.x) reinterpret_cast<uint4*>(fw)[i] = __ldg(reinterpret_cast<const uint4*>(frag) + i);
     __syncthreads();
-    SR_PDL_SYNC();
+    pdl_wait_and_release();
     const int lane = threadIdx.x & 31, g = lane >> 2, tq = lane & 3;
     const long long nblk = (p.P + 15) / 16;
     for (long long blk = (long long)blockIdx.x * 4 + (threadIdx.x >> 5); blk < nblk; blk += (long long)gridDim.x * 4) {
@@ -717,8 +672,8 @@ __global__ void __launch_bounds__(128) sft_mma_kernel(const __grid_constant__ Sf
             const float2 b0 = __ldg(reinterpret_cast<const float2*>(p.cond + pixB * 32 + 16 * ks + 2 * tq));
             const float2 a1 = __ldg(reinterpret_cast<const float2*>(p.cond + pixA * 32 + 16 * ks + 8 + 2 * tq));
             const float2 b1 = __ldg(reinterpret_cast<const float2*>(p.cond + pixB * 32 + 16 * ks + 8 + 2 * tq));
-            ca[ks][0] = sr_pack_sat(a0.x, a0.y); ca[ks][1] = sr_pack_sat(b0.x, b0.y);
-            ca[ks][2] = sr_pack_sat(a1.x, a1.y); ca[ks][3] = sr_pack_sat(b1.x, b1.y);
+            ca[ks][0] = h2_sat(a0.x, a0.y); ca[ks][1] = h2_sat(b0.x, b0.y);
+            ca[ks][2] = h2_sat(a1.x, a1.y); ca[ks][3] = h2_sat(b1.x, b1.y);
         }
         uint32_t as[2][4], ah[2][4];
         sft_hidden(fw, L, ca, g, tq, as, ah);
@@ -750,8 +705,8 @@ __global__ void __launch_bounds__(128) sft_mma_kernel(const __grid_constant__ Sf
                     *reinterpret_cast<float2*>(p.dst_f + pixB * 64 + ch) = make_float2(y[2] * p.res_scale + r.x, y[3] * p.res_scale + r.y);
                 }
             } else {
-                if (inA) *reinterpret_cast<uint32_t*>(p.dst_h + pixA * p.dst_cstride + p.dst_c0 + ch) = sr_pack_sat(y[0], y[1]);
-                if (inB) *reinterpret_cast<uint32_t*>(p.dst_h + pixB * p.dst_cstride + p.dst_c0 + ch) = sr_pack_sat(y[2], y[3]);
+                if (inA) *reinterpret_cast<uint32_t*>(p.dst_h + pixA * p.dst_cstride + p.dst_c0 + ch) = h2_sat(y[0], y[1]);
+                if (inB) *reinterpret_cast<uint32_t*>(p.dst_h + pixB * p.dst_cstride + p.dst_c0 + ch) = h2_sat(y[2], y[3]);
             }
         }
     }
@@ -791,7 +746,7 @@ __global__ void __launch_bounds__(128) condnet_kernel(const __grid_constant__ Co
     __syncthreads();
     const float* c0 = sw; const float* b0 = c0 + 576; const float* c2 = b0 + 64; const float* b2 = c2 + 4096;
     const float* c4 = b2 + 64; const float* b4 = c4 + 4096; const float* c6 = b4 + 64; const float* b6 = c6 + 2048;
-    SR_PDL_SYNC();
+    pdl_wait_and_release();
     const long long pix = (long long)p.y_lo * p.W + (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (pix >= (long long)p.y_hi * p.W) return;
     const int y = (int)(pix / p.W), x = (int)(pix - (long long)y * p.W);
@@ -856,7 +811,7 @@ __global__ void __launch_bounds__(128) condnet_kernel(const __grid_constant__ Co
 #pragma unroll
         for (int k = 0; k < 64; ++k) v = fmaf(c6[o * 64 + k], a[k], v);
         p.cond_out[pix * 32 + o] = v;
-        if (p.cond16) p.cond16[pix * 32 + o] = __low2half(sr_h2sat(v, 0.f));   // operand of the fused SFT epilogues, saturated
+        if (p.cond16) p.cond16[pix * 32 + o] = __ushort_as_half((unsigned short)h2_sat(v, 0.f));   // operand of the fused SFT epilogues
     }
 }
 
@@ -923,9 +878,9 @@ struct CondMmaParams { const float* cond_in; const unsigned char* wblk; float* c
 // rounding to inf would make lo = -inf and the next MMA NaN).
 __device__ __forceinline__ void cnm_split_frag(const float (&c0)[4], const float (&c1)[4], uint32_t (&ah)[4], uint32_t (&al)[4]) {
     auto pk = [](float x, float y, uint32_t& hi, uint32_t& lo) {
-        hi = sr_pack_sat(x, y);
+        hi = h2_sat(x, y);
         const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
-        lo = sr_pack_sat(x - hf.x, y - hf.y);
+        lo = h2_sat(x - hf.x, y - hf.y);
     };
     pk(c0[0], c0[1], ah[0], al[0]); pk(c0[2], c0[3], ah[1], al[1]);
     pk(c1[0], c1[1], ah[2], al[2]); pk(c1[2], c1[3], ah[3], al[3]);
@@ -945,9 +900,9 @@ __device__ __forceinline__ void cnm_layer(const unsigned char* sm, int offh, int
             const __half* wh = Wh + (8 * j + g) * CNM_PITCH + 16 * ks + 2 * tq;
             const __half* wl = Wl + (8 * j + g) * CNM_PITCH + 16 * ks + 2 * tq;
             const uint32_t bh0 = *reinterpret_cast<const uint32_t*>(wh), bh1 = *reinterpret_cast<const uint32_t*>(wh + 8);
-            sr_hmma(c[j], al[ks], bh0, bh1);                     // small terms first
-            sr_hmma(c[j], ah[ks], *reinterpret_cast<const uint32_t*>(wl), *reinterpret_cast<const uint32_t*>(wl + 8));
-            sr_hmma(c[j], ah[ks], bh0, bh1);
+            mma_16816(c[j], al[ks], bh0, bh1);                     // small terms first
+            mma_16816(c[j], ah[ks], *reinterpret_cast<const uint32_t*>(wl), *reinterpret_cast<const uint32_t*>(wl + 8));
+            mma_16816(c[j], ah[ks], bh0, bh1);
         }
     }
 }
@@ -978,11 +933,11 @@ __device__ __forceinline__ void cnm_tail(const unsigned char* csm, const CnmLayo
         const int ch = 8 * j + 2 * tq;
         if (inA) {
             *reinterpret_cast<float2*>(p.cond_out + pixA * 32 + ch) = make_float2(o[j][0], o[j][1]);
-            if (p.cond16) *reinterpret_cast<__half2*>(p.cond16 + pixA * 32 + ch) = sr_h2sat(o[j][0], o[j][1]);
+            if (p.cond16) *reinterpret_cast<uint32_t*>(p.cond16 + pixA * 32 + ch) = h2_sat(o[j][0], o[j][1]);
         }
         if (inB) {
             *reinterpret_cast<float2*>(p.cond_out + pixB * 32 + ch) = make_float2(o[j][2], o[j][3]);
-            if (p.cond16) *reinterpret_cast<__half2*>(p.cond16 + pixB * 32 + ch) = sr_h2sat(o[j][2], o[j][3]);
+            if (p.cond16) *reinterpret_cast<uint32_t*>(p.cond16 + pixB * 32 + ch) = h2_sat(o[j][2], o[j][3]);
         }
     }
 }
@@ -992,7 +947,7 @@ __global__ void __launch_bounds__(128) condnet_mma_kernel(const __grid_constant_
     const CnmLayout L = cnm_layout();
     for (int i = threadIdx.x; i < L.total / 16; i += blockDim.x) reinterpret_cast<uint4*>(csm)[i] = __ldg(reinterpret_cast<const uint4*>(p.wblk) + i);
     __syncthreads();
-    SR_PDL_SYNC();
+    pdl_wait_and_release();
     const int lane = threadIdx.x & 31, g = lane >> 2, tq = lane & 3;
     const long long p0 = (long long)p.y_lo * p.W, pend = (long long)p.y_hi * p.W;
     const long long nblk = (pend - p0 + 15) / 16;
@@ -1048,7 +1003,7 @@ __global__ void __launch_bounds__(256, 1) condnet_wide_mma_kernel(const __grid_c
     const CnmLayout L = cnm_layout();
     for (int i = threadIdx.x; i < cnw_bytes() / 16; i += blockDim.x) reinterpret_cast<uint4*>(csm)[i] = __ldg(reinterpret_cast<const uint4*>(p.wblk) + i);
     __syncthreads();
-    SR_PDL_SYNC();
+    pdl_wait_and_release();
     const int lane = threadIdx.x & 31, g = lane >> 2, tq = lane & 3, nwarps = blockDim.x >> 5;
     const long long p0 = (long long)p.y_lo * p.W, pend = (long long)p.y_hi * p.W;
     const long long nblk = (pend - p0 + 15) / 16, plane = (long long)p.H * p.W;
@@ -1090,9 +1045,9 @@ __global__ void __launch_bounds__(256, 1) condnet_wide_mma_kernel(const __grid_c
                     const __half* wh = W0h + (8 * j + g) * CNW_PITCH + k0;
                     const __half* wl = W0l + (8 * j + g) * CNW_PITCH + k0;
                     const uint32_t bh0 = *reinterpret_cast<const uint32_t*>(wh), bh1 = *reinterpret_cast<const uint32_t*>(wh + 8);
-                    sr_hmma(c[j], al, bh0, bh1);                  // small terms first
-                    sr_hmma(c[j], ah, *reinterpret_cast<const uint32_t*>(wl), *reinterpret_cast<const uint32_t*>(wl + 8));
-                    sr_hmma(c[j], ah, bh0, bh1);
+                    mma_16816(c[j], al, bh0, bh1);                  // small terms first
+                    mma_16816(c[j], ah, *reinterpret_cast<const uint32_t*>(wl), *reinterpret_cast<const uint32_t*>(wl + 8));
+                    mma_16816(c[j], ah, bh0, bh1);
                 }
             }
         }
@@ -1109,7 +1064,7 @@ __global__ void __launch_bounds__(256, 1) condnet_wide_mma_kernel(const __grid_c
 
 // planar fp32 [C,H,W] -> NHWC fp16 [H,W,32] (zero padded)
 __global__ void nchw_to_nhwc32_kernel(const float* __restrict__ src, __half* __restrict__ dst, int C, long long P) {
-    SR_PDL_SYNC();
+    pdl_wait_and_release();
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P * 32) return;
     const long long pix = i >> 5;
@@ -1372,18 +1327,26 @@ static k4_encode_tiled_fn sr_encode_tiled() {
     return fn;
 }
 
+// Tensor map of a rank-2 or rank-3 fp16 tensor at `base`: dense boxes (unit element strides), no interleave, 128-byte
+// L2 promotion, and zeros for the elements of a box that lie outside the tensor (the convolutions' padding).  False when
+// the driver has no cuTensorMapEncodeTiled or rejects the map.
+static bool encode_f16_tmap(CUtensorMap* map, const void* base, cuuint32_t rank, const cuuint64_t* gdim, const cuuint64_t* gstride,
+                            const cuuint32_t* box, CUtensorMapSwizzle swizzle) {
+    k4_encode_tiled_fn enc = sr_encode_tiled();
+    const cuuint32_t estr[3] = {1, 1, 1};
+    return enc && enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<void*>(base), gdim, gstride, box, estr,
+                      CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
 // (channel, x, y) view of the NHWC fp16 source starting at channel src_c0; box = one 8-channel halo plane
 static bool sr_make_tmap(const ConvParams& p, CUtensorMap* tm) {
-    k4_encode_tiled_fn enc = sr_encode_tiled();
-    if (!enc) return false;
     const cuuint64_t gdim[3] = {(cuuint64_t)p.cin, (cuuint64_t)p.W, (cuuint64_t)p.H};
     const cuuint64_t gstride[2] = {(cuuint64_t)p.src_cstride * 2, (cuuint64_t)p.W * p.src_cstride * 2};
     const cuuint32_t box[3] = {8, (cuuint32_t)WS_HX, (cuuint32_t)SR_HY};
-    const cuuint32_t estr[3] = {1, 1, 1};
-    void* base = const_cast<__half*>(p.src + p.src_c0);
+    const __half* base = p.src + p.src_c0;
     if (((uintptr_t)base & 15) || (gstride[0] & 15)) return false;
-    return enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, base, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    return encode_f16_tmap(tm, base, 3, gdim, gstride, box, CU_TENSOR_MAP_SWIZZLE_NONE);
 }
 
 static bool sr_no_tma() {
@@ -1422,26 +1385,21 @@ int launch_conv_ws(ConvParams p, cudaStream_t s, int sel, int* used) {
 template <int N>
 int launch_conv_k64(ConvParams p, const __half* wrows, cudaStream_t s) {
     using C = K64Cfg<N>;
-    k4_encode_tiled_fn enc = sr_encode_tiled();
-    if (!enc) return K4_ERR_UNSUPPORTED;
+    if (!sr_encode_tiled()) return K4_ERR_UNSUPPORTED;
     if (int st = sr_set_smem(conv3x3_k64_kernel<N>, 6 + sr_bit_n(N), C::SMEM)) return st;
     const int sms = sr_dev()->sms;
     alignas(64) CUtensorMap ta, tb;
     {
         const cuuint64_t gdim[3] = {64, (cuuint64_t)p.W, (cuuint64_t)p.H};
         const cuuint64_t gstr[2] = {(cuuint64_t)p.src_cstride * 2, (cuuint64_t)p.W * p.src_cstride * 2};
-        const cuuint32_t box[3] = {64, (cuuint32_t)K64_HX, (cuuint32_t)SR_HY}, es[3] = {1, 1, 1};
-        if (enc(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(p.src + p.src_c0), gdim, gstr, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return K4_ERR_UNSUPPORTED;
+        const cuuint32_t box[3] = {64, (cuuint32_t)K64_HX, (cuuint32_t)SR_HY};
+        if (!encode_f16_tmap(&ta, p.src + p.src_c0, 3, gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_128B)) return K4_ERR_UNSUPPORTED;
     }
     {
         const cuuint64_t gdim[2] = {64, (cuuint64_t)p.ntaps * N};
         const cuuint64_t gstr[1] = {128};
-        const cuuint32_t box[2] = {64, (cuuint32_t)N}, es[2] = {1, 1};
-        if (enc(&tb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(wrows), gdim, gstr, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return K4_ERR_UNSUPPORTED;
+        const cuuint32_t box[2] = {64, (cuuint32_t)N};
+        if (!encode_f16_tmap(&tb, wrows, 2, gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_128B)) return K4_ERR_UNSUPPORTED;
     }
     const int tiles = ((p.W + K64_TX - 1) / K64_TX) * ((p.y_hi - p.y_lo + SR_TY - 1) / SR_TY);
     if (tiles <= 0) return K4_OK;

@@ -255,7 +255,7 @@ def test_f16x3_keeps_the_lo_parts_exactly(cuda_device, spec):
 
 @pytest.mark.parametrize('spec', MODELS, ids=MODEL_IDS)
 def test_wgmma_inputs_saturate_to_fp16_max(cuda_device, spec):
-    """Inputs beyond the fp16 range enter the wgmma rows as +-65504 (pack2 is cvt.rn.satfinite), never as inf."""
+    """Inputs beyond the fp16 range enter the wgmma rows as +-65504 (h2_sat is cvt.rn.satfinite), never as inf."""
     rng = np.random.default_rng(11)
     name, kind, c, vpe, spe, width, direct, cid = spec
     dim0 = dim0_of(kind, c, vpe, spe, direct)
