@@ -137,6 +137,17 @@ __global__ void pack_tc_bias_kernel(const float* __restrict__ b, unsigned char* 
     }
     *reinterpret_cast<__half*>(dst + tc_canon_off(n, k >> 3, 2) + (k & 7) * 2) = __float2half_rn(v);
 }
+// layer 1's bias inside K (k4_ws_bias_col): W1 tile [npad][kpad] column col = fp16(b), col + 1 = fp16(b - col), the split
+// of pack_tc_bias_kernel; the A rows hold 1.0 in both columns
+__global__ void pack_tc_bias_col_kernel(const float* __restrict__ b, unsigned char* __restrict__ dst, int n_out, int kpad, int col) {
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n >= n_out) return;
+    const float bb = b[n];
+    const __half hi = __float2half_rn(bb);
+    __half* p = reinterpret_cast<__half*>(dst + tc_canon_off(n, col >> 3, kpad >> 3) + (col & 7) * 2);
+    p[0] = hi;
+    p[1] = __float2half_rn(bb - __half2float(hi));
+}
 __global__ void pack_tc_ones_kernel(unsigned char* __restrict__ dst) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= 128 * 16) return;
@@ -271,10 +282,18 @@ extern "C" int k4_scene_create(const k4_scene_desc* d, k4_stream_t stream, k4_sc
     v.kind = d->kind;
     v.X = d->world_size[0]; v.Y = d->world_size[1]; v.Z = d->world_size[2];
     v.C = d->k0_dim; v.Cpad = round_up(d->k0_dim, 4);
-    // wgmma config this model runs on (k4_ws_cfgs.h): its k0 copy is padded to the config's channel count
+    // wgmma config this model runs on (k4_ws_cfgs.h): its k0 copy is padded to the config's channel count.
+    // K4_WS_CONFIG=<id> (A-B / tests): that entry instead of the first covering one; one that does not cover the model
+    // leaves the scene without a wgmma build.
+    int want_cfg = -1;
+    if (const char* e = getenv("K4_WS_CONFIG")) {      // a value that is not a whole non-negative number: no override
+        char* end = nullptr;
+        const long id = strtol(e, &end, 10);
+        if (end != e && *end == '\0' && id >= 0 && id < 1000) want_cfg = (int)id;
+    }
     const K4WsCfg* wcfg = (d->rgbnet_depth > 0)
         ? k4_ws_pick(d->kind, d->k0_dim, d->viewbase_pe, d->kind == K4_KIND_DMPIGO ? d->spatial_pe : 0, d->rgbnet_width,
-                     d->kind == K4_KIND_DVGO ? (d->rgbnet_direct != 0) : 1, d->rgbnet_depth)
+                     d->kind == K4_KIND_DVGO ? (d->rgbnet_direct != 0) : 1, d->rgbnet_depth, want_cfg)
         : nullptr;
     if (wcfg && round_up(wcfg->C, 4) > v.Cpad) v.Cpad = round_up(wcfg->C, 4);
     v.tc_cfg = -1; v.tc_exact = 0;
@@ -425,7 +444,10 @@ extern "C" int k4_scene_create(const k4_scene_desc* d, k4_stream_t stream, k4_sc
                 pack_tc_weight_kernel<<<(wm * wm + 255) / 256, 256, 0, s>>>(d->d_rgbnet_weight[1], blob + BL.off_w2, wm, wm, w, nullptr);
                 // W3 / B3: output channel c at operand row (accumulator column) 2c, for mlp_batch_wgmma's epilogue
                 pack_tc_weight_kernel<<<(3 * wm + 255) / 256, 256, 0, s>>>(d->d_rgbnet_weight[2], blob + BL.off_w3, 3, wm, w, nullptr, 2);
-                pack_tc_bias_kernel<<<(w * 16 + 255) / 256, 256, 0, s>>>(d->d_rgbnet_bias[0], blob + BL.off_b1, wm, w);
+                if (k4_ws_bias_col(c) >= 0)
+                    pack_tc_bias_col_kernel<<<(wm + 127) / 128, 128, 0, s>>>(d->d_rgbnet_bias[0], blob + BL.off_w1, wm, kpad, k4_ws_bias_col(c));
+                else
+                    pack_tc_bias_kernel<<<(w * 16 + 255) / 256, 256, 0, s>>>(d->d_rgbnet_bias[0], blob + BL.off_b1, wm, w);
                 pack_tc_bias_kernel<<<(w * 16 + 255) / 256, 256, 0, s>>>(d->d_rgbnet_bias[1], blob + BL.off_b2, wm, w);
                 pack_tc_bias_kernel<<<1, 256, 0, s>>>(d->d_rgbnet_bias[2], blob + BL.off_b3, 3, 16, 2);
                 pack_tc_ones_kernel<<<8, 256, 0, s>>>(blob + BL.off_ones);
@@ -642,6 +664,14 @@ int testing_rgbnet_mma(const K4Dev& v, const k4_rgbnet_test_args* a, cudaStream_
 }
 
 }  // namespace
+
+extern "C" int k4_testing_ws_row_layout(int32_t config, int32_t* out) {
+    int32_t v[4];
+    if (!out) return K4_ERR_INVALID_ARG;
+    const int st = k4_ws_row_layout(config, v);
+    for (int i = 0; i < 4; ++i) out[i] = st == K4_OK ? v[i] : 0;
+    return st;
+}
 
 extern "C" int k4_testing_rgbnet(const k4_scene* sc, const k4_rgbnet_test_args* a, int32_t* group_rows, k4_stream_t stream) {
     if (group_rows) *group_rows = 0;

@@ -66,8 +66,9 @@ struct TcBlobLayout {
     int off_w1, off_w2, off_w3, off_b1, off_b2, off_b3, off_ones, total;
 };
 // W1 [W][kpad], W2 [W][W], W3 [16][W], bias tiles B1/B2 [W][16], B3 [16][16] (col 0 = fp16(b),
-// col 1 = fp16(b - col0)), ONES [128][16] (cols 0,1 = 1): every layer's bias is one extra K=16 MMA.  Output channel c of
-// the last layer is row 2c of W3 and B3 (the other rows are zero), for the epilogue of mlp_batch_wgmma.
+// col 1 = fp16(b - col0)), ONES [128][16] (cols 0,1 = 1): a layer's bias is one extra K=16 MMA -- but for layer 1 of a
+// config with two spare K columns (k4_ws_bias_col), whose bias hi / lo sit in those columns of W1 (B1 stays zero).
+// Output channel c of the last layer is row 2c of W3 and B3 (the other rows are zero), for the epilogue of mlp_batch_wgmma.
 __host__ __device__ inline TcBlobLayout tc_blob_layout(int kpad, int w) {
     TcBlobLayout L;
     int o = 0;
@@ -133,6 +134,8 @@ int k4_launch_march(const k4_scene* sc, const K4RenderParams& rp, int mlp_mode, 
 int k4_launch_march_tc(const k4_scene* sc, K4RenderParams rp, cudaStream_t st);   // K4_ERR_UNSUPPORTED if the shape has no wgmma build
 bool k4_tc_supported(const K4Dev& v);
 bool k4_ws_supported(const K4Dev& v);
+// k4_testing_ws_row_layout: the compile-time row layout of K4_WS_CFG_LIST entry `id` (k4_march_ws.cu)
+int k4_ws_row_layout(int id, int32_t out[4]);
 // warp-specialised variant (same shapes).  phases != NULL runs the profiled kernel (k4_testing_march_phases), which
 // writes the phase counters of at most max_ctas CTAs there; *n_ctas (may be NULL) receives the CTA count
 int k4_launch_march_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st, unsigned long long* phases = nullptr,

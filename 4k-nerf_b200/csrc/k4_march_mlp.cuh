@@ -6,9 +6,11 @@
 //       relu is the fused cvt.rn.relu.f16x2, gauss / lkrelu are evaluated in fp32 first: mlp_act_h2)
 //   L2  acc[64 x W] = H1(registers) * W2(smem) + bias                  wgmma RS
 //   E2  same repack -> H2
-//   L3  acc[64 x 16] = H2(registers) * W3(smem) + bias -> sigmoid -> weight -> shared-memory atomicAdd into the ray
-// Every bias is one more K=16 MMA against the constant ONES tile of the operand blob (bias = fp16 hi + fp16 lo
-// columns), as in the blob's layout (tc_blob_layout).
+//   L3  acc[64 x 8] = H2(registers) * W3(smem) + bias -> sigmoid -> weight -> shared-memory atomicAdd into the ray
+// A bias is one more K=16 MMA against the constant ONES tile of the operand blob (bias = fp16 hi + fp16 lo columns), as
+// in the blob's layout (tc_blob_layout) -- except layer 1's where the config has room for it inside K (TcCfg::BIASC):
+// there the ring rows carry fp16 1.0 in two padding columns and W1 the bias hi / lo in the same columns, so the bias
+// products ride in L1's last k16 step.
 #pragma once
 #include "k4_march_common.cuh"
 #include "k4_ptx.cuh"
@@ -69,31 +71,40 @@ struct PhaseClock {
 };
 
 // What the epilogue needs of a lane's two rows of a 64-row half (rows g and g + 8 of its warp's 16): channel t's logit
-// (o[0] / o[2] of the m64n16 accumulator, diffuse term added), the sample weight and the owning ray; owner -1 for a row
+// (o[0] / o[2] of the m64n8 accumulator, diffuse term added), the sample weight and the owning ray; owner -1 for a row
 // beyond `valid` and for lane t == 3, which has no channel.
 struct MlpEpiRows {
     float logit[2], w[2];
     int owner[2];
 };
 
+// The rows' weights, owners and diffuse logits (into logit[], 0 for DIRECT): shared-memory reads that do not depend on L3,
+// issued while its MMAs run.
 template <bool DIRECT>
-__device__ __forceinline__ MlpEpiRows mlp_epi_rows(const float (&o)[8], int row0, int valid, unsigned slot0, const float* qw,
-                                                   const unsigned char* qowner, const float* qdiff, int t) {
+__device__ __forceinline__ MlpEpiRows mlp_epi_inputs(int row0, int valid, unsigned slot0, const float* qw, const unsigned char* qowner,
+                                                     const float* qdiff, int t) {
     MlpEpiRows e;
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {
         const int row = row0 + 8 * rr;
-        e.logit[rr] = o[2 * rr];
+        e.logit[rr] = 0.f;
         e.w[rr] = 0.f;
         e.owner[rr] = -1;
         if (t < 3 && row < valid) {
             const unsigned slot = slot0 + (unsigned)row;
-            if (!DIRECT) e.logit[rr] = __fadd_rn(e.logit[rr], qdiff[slot * 3 + t]);      // rgb_logit + k0_diffuse
+            if (!DIRECT) e.logit[rr] = qdiff[slot * 3 + t];
             e.w[rr] = qw[slot];
             e.owner[rr] = qowner[slot];
         }
     }
     return e;
+}
+
+// ... and the retired L3 accumulator: logit = rgb_logit (+ k0_diffuse)
+template <bool DIRECT>
+__device__ __forceinline__ void mlp_epi_logits(MlpEpiRows& e, const float (&o)[4]) {
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) e.logit[rr] = DIRECT ? o[2 * rr] : __fadd_rn(o[2 * rr], e.logit[rr]);
 }
 
 // w * sigmoid(logit) of the rows, added to racc[3 * owner + t].  A shared-memory float atomicAdd is a compare-and-swap
@@ -115,14 +126,16 @@ __device__ __forceinline__ void mlp_epilogue(const MlpEpiRows& e, float* racc, i
 // first half's epilogue under the second half's L1 MMAs instead keeps the accumulator, the epilogue and its inputs
 // live at once: the 128-wide configurations then need 150 registers of the 128 and ptxas serialises the wgmmas (C7518).
 // `mark` receives the phase boundaries (PhaseClock).  ACT: the hidden activation of E1 / E2 (K4_ACT_*), act_c its
-// constant (K4Dev::act_c; unused by relu).
-template <int W, int KPAD, bool DIRECT, int ACT, class Consumed, class Mark = NoPhases>
+// constant (K4Dev::act_c; unused by relu).  BIASC: the first of the two columns of the A tile that hold fp16 1.0 and of W1
+// that hold layer 1's bias hi / lo (TcCfg::BIASC), -1 where layer 1 adds its bias against the ONES tile.
+template <int W, int KPAD, bool DIRECT, int ACT, int BIASC, class Consumed, class Mark = NoPhases>
 __device__ __forceinline__ void mlp_batch_wgmma(uint32_t a_tile, const unsigned char* blob, const TcBlobLayout& BL, int valid,
                                                 unsigned slot0, const float* qw, const unsigned char* qowner, const float* qdiff,
                                                 float* racc, int wt, float act_c, const Consumed& consumed, bool colour_first,
                                                 const Mark& mark = Mark()) {
     constexpr int KCH = KPAD / 8, KCHW = W / 8, NC = W / 64;      // NC: 64-column blocks of a hidden layer
     static_assert(W % 64 == 0, "hidden width");
+    static_assert(BIASC < 0 || (BIASC % 2 == 0 && BIASC + 1 < KPAD), "layer-1 bias columns");
     const int warp = wt >> 5, g = (wt & 31) >> 2, t = wt & 3;
     const uint32_t blob_s = smem_u32(blob);
     const uint32_t w1 = blob_s + BL.off_w1, w2 = blob_s + BL.off_w2, w3 = blob_s + BL.off_w3;
@@ -143,7 +156,7 @@ __device__ __forceinline__ void mlp_batch_wgmma(uint32_t a_tile, const unsigned 
 #pragma unroll
             for (int k = 0; k < KPAD / 16; ++k)
                 wgmma_ss(acc, wg_desc(a_half + k * 256, 128, KCH * 128), wg_desc(w1 + k * 256, 128, KCH * 128), k > 0);
-            wgmma_ss(acc, d_ones, wg_desc(b1, 128, 256), 1);
+            if constexpr (BIASC < 0) wgmma_ss(acc, d_ones, wg_desc(b1, 128, 256), 1);
             wg_commit();
             wg_wait<0>();
             wg_fence_acc(acc);
@@ -166,18 +179,20 @@ __device__ __forceinline__ void mlp_batch_wgmma(uint32_t a_tile, const unsigned 
             for (int nc = 0; nc < NC; ++nc) mlp_repack<ACT>(*reinterpret_cast<const float (*)[32]>(acc + 32 * nc), h2 + 4 * nc, act_c);
             mark(K4_PH_L_REPACK);
         }
-        float o[8];
+        // W3 / B3 hold output channel c in column 2c (k4_scene_create), so channel c of rows g / g+8 is o[0] / o[2] of lane
+        // t = c: three lanes of each quad share the epilogue.  Columns 0..7 of the 16-row tiles are all there is, so L3
+        // runs at N = 8.
+        float o[4];
         wg_fence();
 #pragma unroll
         for (int k = 0; k < W / 16; ++k) wgmma_rs(o, h2[k], wg_desc(w3 + k * 256, 128, KCHW * 128), k > 0);
         wgmma_ss(o, d_ones, wg_desc(b3, 128, 256), 1);
         wg_commit();
+        pend = mlp_epi_inputs<DIRECT>(mh * 64 + warp * 16 + g, valid, slot0, qw, qowner, qdiff, t);
         wg_wait<0>();
         wg_fence_acc(o);
+        mlp_epi_logits<DIRECT>(pend, o);
         mark(K4_PH_L_L3);
-        // W3 / B3 hold output channel c in column 2c (k4_scene_create), so channel c of rows g / g+8 is o[0] / o[2] of lane
-        // t = c: three lanes of each quad share the epilogue
-        pend = mlp_epi_rows<DIRECT>(o, mh * 64 + warp * 16 + g, valid, slot0, qw, qowner, qdiff, t);
         if (mh + 1 < halves) {
             mlp_epilogue(pend, racc, t);
             mark(K4_PH_L_EPILOGUE);

@@ -24,7 +24,8 @@ __device__ __forceinline__ void stage_blob(unsigned char* blob, const void* src,
 // ---------------------------------------------------------------------------------------------
 // A model shape one of the kernels is built for: an entry of K4_WS_CFG_LIST (k4_ws_cfgs.h) for k4_march_ws.cu, CfgA /
 // CfgB (ID -1) for k4_march_tc.cu.  Row layout of the A operand (fp16): [per-sample features: k0 channels K0OFF..C-1, MPI
-// position + its sin/cos, zero-padded to an even count NS][view embedding: v, sin, cos (NVEMB)][zeros to KPAD].
+// position + its sin/cos, zero-padded to an even count NS][view embedding: v, sin, cos (NVEMB)][zeros to KPAD, but for
+// layer 1's bias ones in columns BIASC, BIASC + 1].
 // TILES: 128-row tiles of a marcher group's ring.  VWS: the marcher keeps its ray's packed view embedding in shared
 // memory (WG_VW) rather than in registers.
 // ---------------------------------------------------------------------------------------------
@@ -45,6 +46,14 @@ struct TcCfg {
     static constexpr int KCH = KPAD / 8;                // 16-byte chunks per A row
     static constexpr int NVW = (NVEMB + 1) / 2;         // packed per-ray words
     static constexpr int TILE_BYTES = 128 * KPAD * 2;
+    // Layer 1's bias inside K: the first even column at or past DIM0, if it and the next one lie below KPAD, else -1
+    // (k4_ws_bias_col).  Row word BIASW = NS/2 + NVW, the first padding word, holds fp16 1.0 in both halves, W1 the
+    // bias hi / lo (mlp_batch_wgmma).  BIAS_STORED: the row store writes BIASW's chunk anyway and puts the word there;
+    // otherwise the chunk is never written and the word is set once, when the ring is zeroed (bias_ones_ring).
+    static constexpr int BIASC = (((DIM0 + 1) & ~1) + 1 < KPAD) ? ((DIM0 + 1) & ~1) : -1;
+    static constexpr int BIASW = BIASC >= 0 ? BIASC / 2 : -1;
+    static constexpr bool BIAS_STORED = BIASC >= 0 && (BIASW % 4) != 0;
+    static_assert(BIASC < 0 || BIASW == NS / 2 + NVW, "the bias word is the row's first padding word");
     static_assert(W == 128 || W == 64, "hidden width");
     static_assert(DIRECT || KIND == K4_KIND_DVGO, "the diffuse term exists in DirectVoxGO only");
     // shared memory map: [blob][marcher group 0][marcher group 1][weight mbarrier]; offsets WG_* inside a group's block
@@ -63,6 +72,22 @@ struct TcCfg {
     static constexpr int PROF_SMEM = SMEM + 4 * PhaseClock::WORDS * 8;   // + the phase counters of a profiled kernel
     static_assert(PROF_SMEM <= 227 * 1024, "shared memory of one block");
 };
+
+constexpr uint32_t H2_ONES = 0x3C003C00u;   // fp16x2 (1.0, 1.0)
+
+// Word j of a ring row outside the sample's features and view embedding: the bias ones or zero padding.
+template <class Cfg>
+__device__ __forceinline__ uint32_t row_pad_word(int j) { return j == Cfg::BIASW ? H2_ONES : 0u; }
+
+// The bias ones of every row of a freshly zeroed ring of `rows` rows at `ring`, where the row store never writes them
+// (!Cfg::BIAS_STORED).  Called by the 128 threads of one warpgroup after the zeroing is visible to them.
+template <class Cfg>
+__device__ __forceinline__ void bias_ones_ring(unsigned char* ring, int rows, int wt) {
+    if constexpr (Cfg::BIASC >= 0 && !Cfg::BIAS_STORED)
+        for (int r = wt; r < rows; r += TC_WG)
+            *reinterpret_cast<uint32_t*>(ring + (r >> 7) * Cfg::TILE_BYTES + tc_canon_off(r & 127, Cfg::BIASC >> 3, Cfg::KCH) +
+                                         (Cfg::BIASC & 7) * 2) = H2_ONES;
+}
 
 // ---------------------------------------------------------------------------------------------
 // per ray

@@ -55,6 +55,7 @@ k4_march_tc_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
         for (int i = wt; i < (Cfg::WG_MISC + 32) / 4; i += TC_WG) z[i] = 0u;
     }
     __syncthreads();
+    bias_ones_ring<Cfg>(wgb, TC_RING, wt);
     if (tid == 0) stage_blob(blob, s.tc_blob, BL.total, wbar);
     mbar_wait(wbar, 0);
     const uint32_t a_ring_s = smem_u32(wgb);
@@ -69,7 +70,7 @@ k4_march_tc_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
         fence_proxy_async();
         named_bar(wg + 1);
         if (wt == 0) ++n_batches;
-        mlp_batch_wgmma<W, KPAD, true, ACT>(a_tile, blob, BL, valid, head & (TC_RING - 1), qw, qowner, nullptr, racc, wt, s.act_c,
+        mlp_batch_wgmma<W, KPAD, true, ACT, Cfg::BIASC>(a_tile, blob, BL, valid, head & (TC_RING - 1), qw, qowner, nullptr, racc, wt, s.act_c,
                                             [] {}, true);
     };
 
@@ -141,7 +142,7 @@ k4_march_tc_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
                         for (int j = 0; j < KPAD / 2; ++j) {
                             if (j < Cfg::NS / 2) row[j] = h2_sat(f[2 * j], f[2 * j + 1]);
                             else if (j < Cfg::NS / 2 + Cfg::NVW) row[j] = vw[j - Cfg::NS / 2];
-                            else row[j] = 0u;
+                            else row[j] = row_pad_word<Cfg>(j);
                         }
                         unsigned char* rowp = wgb + (slot >> 7) * Cfg::TILE_BYTES + tc_canon_off((int)(slot & 127), 0, KCH);
 #pragma unroll

@@ -64,6 +64,7 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
         for (int i = wt; i < (Cfg::WG_MISC + (int)sizeof(WgCtl)) / 4; i += TC_WG) z[i] = 0u;
     }
     __syncthreads();
+    if (tid < 256) bias_ones_ring<Cfg>(wg_base(wg), Cfg::RING, wt);
     if (tid == 0) {
         mbar_init(wbar, 1);
         for (int g = 0; g < 2; ++g) {
@@ -103,10 +104,10 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
             const int valid = *reinterpret_cast<volatile int*>(&c->valid[tile]);
             const bool last = *reinterpret_cast<volatile int*>(&c->last[tile]) != 0;
             if (PROF)
-                mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0, ACT>(ring_s + tile * Cfg::TILE_BYTES, blob, BL, valid, tile * 128u, qw,
+                mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0, ACT, Cfg::BIASC>(ring_s + tile * Cfg::TILE_BYTES, blob, BL, valid, tile * 128u, qw,
                                                                 qowner, qdiff, racc, wt, s.act_c, consumed, last, clk);
             else
-                mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0, ACT>(ring_s + tile * Cfg::TILE_BYTES, blob, BL, valid, tile * 128u, qw,
+                mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0, ACT, Cfg::BIASC>(ring_s + tile * Cfg::TILE_BYTES, blob, BL, valid, tile * 128u, qw,
                                                                 qowner, qdiff, racc, wt, s.act_c, consumed, last);
             ++nb;
         }
@@ -234,7 +235,7 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
                                     const int j = 4 * kc + e;
                                     if (j < Cfg::NS / 2) q[e] = h2_sat(f[Cfg::K0OFF + 2 * j], f[Cfg::K0OFF + 2 * j + 1]);
                                     else if (j < Cfg::NS / 2 + Cfg::NVW) q[e] = vws[(j - Cfg::NS / 2) * 128];
-                                    else q[e] = 0u;
+                                    else q[e] = row_pad_word<Cfg>(j);
                                 }
                                 *reinterpret_cast<uint4*>(rowp + kc * 128) = make_uint4(q[0], q[1], q[2], q[3]);
                             }
@@ -283,6 +284,14 @@ k4_march_ws_kernel(const __grid_constant__ K4Dev s, const __grid_constant__ K4Re
         if (PROF) clk.end(n_sub, phases + ((size_t)blockIdx.x * 4 + wg) * K4_PHASE_SLOTS);
     }
 }
+
+// the blob's W1 carries layer 1's bias where the config's kernels expect it (k4_scene_create packs by k4_ws_bias_col)
+#define K4_X(id, kind, C, vpe, spe, W, direct)                                                                    \
+    static_assert(TcCfg<id, kind, C, vpe, spe, W, direct, TC_TILES, true>::BIASC ==                                \
+                  k4_ws_bias_col(K4WsCfg{id, kind, C, vpe, spe, W, direct}), "layer-1 bias column of config " #id); \
+    static_assert(TcCfg<id, kind, C, vpe, spe, W, direct, TC_TILES, true>::KPAD == k4_ws_kpad(K4WsCfg{id, kind, C, vpe, spe, W, direct}));
+K4_WS_CFG_LIST(K4_X)
+#undef K4_X
 
 // phases: NULL for the production kernel, else the profiled one writes there (room for max_ctas CTAs); *n_ctas: CTAs launched
 template <class Cfg, int ACT>
@@ -340,6 +349,7 @@ k4_test_rgbnet_ws_kernel(const __grid_constant__ K4Dev s, const float* __restric
     for (int k = 0; k < KPAD; ++k) f[k] = 0.f;
     if (wt < valid)
         for (int k = 0; k < s.dim0; ++k) f[__ldg(s.tc_colmap + k)] = xs[r * s.dim0 + k];
+    if (Cfg::BIASC >= 0) f[Cfg::BIASC] = f[Cfg::BIASC + 1] = 1.f;
     unsigned char* rowp = tile + tc_canon_off(wt, 0, KCH);
 #pragma unroll
     for (int kc = 0; kc < KCH; ++kc)
@@ -355,7 +365,7 @@ k4_test_rgbnet_ws_kernel(const __grid_constant__ K4Dev s, const float* __restric
     fence_proxy_async();
     mbar_wait(bar, 0);
     __syncthreads();
-    mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0, ACT>(smem_u32(tile), blob, BL, valid, 0u, qw, qowner, qdiff, racc, wt, s.act_c, [] {}, true);
+    mlp_batch_wgmma<W, KPAD, Cfg::DIRECT != 0, ACT, Cfg::BIASC>(smem_u32(tile), blob, BL, valid, 0u, qw, qowner, qdiff, racc, wt, s.act_c, [] {}, true);
     __syncthreads();
 #pragma unroll
     for (int c = 0; c < 3; ++c) racc_out[3 * (r0 + wt) + c] = racc[3 * wt + c];
@@ -417,3 +427,17 @@ int k4_launch_march_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st, u
 }
 
 bool k4_ws_supported(const K4Dev& v) { return v.tc_blob != nullptr && v.tc_cfg >= 0; }
+
+int k4_ws_row_layout(int id, int32_t out[4]) {
+    switch (id) {
+#define K4_X(id, kind, C, vpe, spe, W, direct)                                                  \
+        case id: {                                                                              \
+            using Cfg = TcCfg<id, kind, C, vpe, spe, W, direct, TC_TILES, true>;                \
+            out[0] = Cfg::DIM0; out[1] = Cfg::KPAD; out[2] = Cfg::BIASC; out[3] = Cfg::BIAS_STORED; \
+            return K4_OK;                                                                       \
+        }
+        K4_WS_CFG_LIST(K4_X)
+#undef K4_X
+        default: return K4_ERR_INVALID_ARG;
+    }
+}

@@ -22,6 +22,19 @@ template <int R> __device__ __forceinline__ void wg_fence_acc(float (&d)[R]) {
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i]) :: "memory");
 }
 
+__device__ __forceinline__ void wgmma_ss(float (&d)[4], uint64_t a, uint64_t b, int scale_d) {   // m64n8k16
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %6, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 {%0, %1, %2, %3}, %4, %5, p, 1, 1, 0, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "l"(a), "l"(b), "r"(scale_d) : "memory");
+}
+__device__ __forceinline__ void wgmma_rs(float (&d)[4], const uint32_t (&a)[4], uint64_t b, int scale_d) {   // m64n8k16, A from registers
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %9, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 {%0, %1, %2, %3}, {%4, %5, %6, %7}, %8, p, 1, 1, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d) : "memory");
+}
+
 __device__ __forceinline__ void wgmma_ss(float (&d)[8], uint64_t a, uint64_t b, int scale_d) {   // m64n16k16
     asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
                  "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n}\n"

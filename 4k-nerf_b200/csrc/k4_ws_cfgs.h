@@ -37,9 +37,17 @@
 struct K4WsCfg { int id, kind, C, vpe, spe, W, direct; };
 
 // per-sample features, padded to an even count (rows are packed as fp16 pairs; the per-ray view embedding follows)
-inline int k4_ws_ns(const K4WsCfg& c) { return (c.direct ? c.C : c.C - 3) + (c.kind == K4_KIND_DMPIGO ? 3 + 6 * c.spe : 0); }
-inline int k4_ws_nsp(const K4WsCfg& c) { return (k4_ws_ns(c) + 1) & ~1; }
-inline int k4_ws_kpad(const K4WsCfg& c) { return (k4_ws_nsp(c) + 3 + 6 * c.vpe + 15) & ~15; }
+constexpr int k4_ws_ns(const K4WsCfg& c) { return (c.direct ? c.C : c.C - 3) + (c.kind == K4_KIND_DMPIGO ? 3 + 6 * c.spe : 0); }
+constexpr int k4_ws_nsp(const K4WsCfg& c) { return (k4_ws_ns(c) + 1) & ~1; }
+constexpr int k4_ws_dim0(const K4WsCfg& c) { return k4_ws_nsp(c) + 3 + 6 * c.vpe; }
+constexpr int k4_ws_kpad(const K4WsCfg& c) { return (k4_ws_dim0(c) + 15) & ~15; }
+// Layer 1's bias rides inside K where the row has two spare columns: the first even column at or past the config's
+// input count, if it and the next one lie below kpad; the rows hold fp16 1.0 there and W1 the bias hi / lo.  -1: no room,
+// layer 1 adds its bias with one more MMA against the ONES tile.  Of the list above, every config with view frequencies
+// folds (1, 3, 4, 10: column 40; 5, 11: 56; 7: 44; 8: 74); 0, 2, 6 and 9 (kpad 16 = 15 inputs + 1) do not.
+constexpr int k4_ws_bias_col(const K4WsCfg& c) {
+    return (((k4_ws_dim0(c) + 1) & ~1) + 1 < k4_ws_kpad(c)) ? ((k4_ws_dim0(c) + 1) & ~1) : -1;
+}
 
 inline const K4WsCfg* k4_ws_cfg_table(int* n) {
     static const K4WsCfg tab[] = {
@@ -51,14 +59,16 @@ inline const K4WsCfg* k4_ws_cfg_table(int* n) {
     return tab;
 }
 
-// first config that covers the model (see the comment at the top), or nullptr
-inline const K4WsCfg* k4_ws_pick(int kind, int C, int vpe, int spe, int width, int direct, int depth) {
+// first config that covers the model (see the comment at the top), or nullptr.  want >= 0: the config of that id if it
+// covers the model, else nullptr (K4_WS_CONFIG, k4_scene_create).
+inline const K4WsCfg* k4_ws_pick(int kind, int C, int vpe, int spe, int width, int direct, int depth, int want = -1) {
     if (depth != 3) return nullptr;
     int n = 0;
     const K4WsCfg* tab = k4_ws_cfg_table(&n);
     if (kind != K4_KIND_DVGO) direct = 1;
     for (int i = 0; i < n; ++i) {
         const K4WsCfg& c = tab[i];
+        if (want >= 0 && c.id != want) continue;
         if (c.kind != kind || c.direct != direct) continue;
         if (C > c.C || (!direct && C < 4) || vpe > c.vpe || spe > c.spe || width > c.W) continue;
         return &c;

@@ -130,6 +130,7 @@ EXPORTS = {
     'k4_scene_device_bytes': (C.c_size_t, [C.c_void_p]),
     'k4_scene_best_mlp_mode': (C.c_int, [C.c_void_p]),
     'k4_scene_ws_config': (C.c_int, [C.c_void_p]),
+    'k4_testing_ws_row_layout': (C.c_int, [C.c_int32, C.POINTER(C.c_int32)]),
     'k4_render_workspace_bytes': (C.c_size_t, [C.c_void_p, C.c_int64]),
     'k4_render_rays': (C.c_int, [C.c_void_p, C.POINTER(RenderArgs), C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_int64, C.POINTER(RenderOut), C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -554,6 +554,19 @@ typedef struct k4_rgbnet_test_args {
 K4_API int k4_testing_rgbnet(const k4_scene* scene, const k4_rgbnet_test_args* args, int32_t* group_rows, k4_stream_t stream);
 
 /*
+ * k4_testing_ws_row_layout: the A-row layout the warp-specialised marcher's kernels are compiled with for the
+ * K4_WS_CFG_LIST entry `config` (csrc/k4_ws_cfgs.h), so that a test can check it without a GPU.  out[4] (host):
+ *   out[0]  the config's inputs per row (its dim0: the padded per-sample features, then the view embedding)
+ *   out[1]  K of layer 1 (dim0 rounded up to 16)
+ *   out[2]  the first of the two columns that hold fp16 1.0 in every row and layer 1's bias hi / lo in W1, so that the
+ *           bias rides inside layer 1's K; -1 where they do not fit below out[1] and layer 1 adds its bias with one more
+ *           MMA against a tile of ones
+ *   out[3]  1 if the marcher's row store writes those ones with every row, 0 if they are written once per ring
+ * An id that is not in the list returns K4_ERR_INVALID_ARG with out zeroed.  Needs no device.
+ */
+K4_API int k4_testing_ws_row_layout(int32_t config, int32_t* out);
+
+/*
  * k4_testing_march_phases: k4_render_rays in mode K4_MLP_TCGEN05_WS, run by the profiled instantiation of the
  * warp-specialised marcher.  It computes what the production kernel computes and, besides, where each warpgroup's SM
  * cycles go: thread 0 of every warpgroup reads the SM clock at each phase boundary and charges the cycles since the
