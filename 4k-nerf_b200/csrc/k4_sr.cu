@@ -1631,11 +1631,20 @@ static inline SrRows sr_rows(int ky0, int ky1, int r, int h) {
     SrRows o; o.lo = ky0 - r < 0 ? 0 : ky0 - r; o.hi = ky1 + r > h ? h : ky1 + r; return o;
 }
 
+// k4_testing_srnet_forward_upto: the steps of a forward are recorded, and it returns after stop_after of them.  The
+// production forward passes no trace.
+struct SrTrace { int stop_after, max_steps, n; k4_sr_step* steps; };
+static inline bool sr_step(SrTrace* t, int kind, int i, int j, int c, int fused) {
+    if (!t) return false;
+    if (t->n < t->max_steps) t->steps[t->n] = k4_sr_step{kind, i, j, c, fused};
+    return ++t->n >= t->stop_after;
+}
+
 static int srnet_forward_roi_impl(const k4_srnet* n, const float* d_x, const float* d_cond, int32_t h, int32_t w,
                                   int32_t keep_y0, int32_t keep_y1, int32_t keep_x0, int32_t keep_x1,
                                   float* d_out, int64_t out_plane_stride, int64_t out_row_stride,
                                   int32_t n_extra, float* const* h_extra,
-                                  void* d_ws, size_t ws_bytes, k4_stream_t stream) {
+                                  void* d_ws, size_t ws_bytes, k4_stream_t stream, SrTrace* tr = nullptr) {
     if (!n || !d_x || !d_cond || !d_out || h <= 0 || w <= 0) return K4_ERR_INVALID_ARG;
     if (n_extra < 0 || n_extra > K4_MAX_PEERS - 1 || (n_extra > 0 && !h_extra)) return K4_ERR_INVALID_ARG;
     for (int e = 0; e < n_extra; ++e) if (!h_extra[e]) return K4_ERR_INVALID_ARG;
@@ -1663,11 +1672,12 @@ static int srnet_forward_roi_impl(const k4_srnet* n, const float* d_x, const flo
     // rows(3 + 5 * 3 * num_block).
     const int nrdb = 3 * n->num_block;
     int st;
-#define SR_DO(x) do { st = (x); if (st != K4_OK) return st; } while (0)
+#define SR_DO(x, ...) do { st = (x); if (st != K4_OK) return st; if (sr_step(tr, __VA_ARGS__)) return K4_OK; } while (0)
     K4_CUDA_TRY(sr_launch(nchw_to_nhwc32_kernel, (unsigned)((P * 32 + 255) / 256), 256, 0, s, d_x, in16, 3, P));
+    if (sr_step(tr, K4_SR_STEP_INPUT, -1, -1, -1, 0)) return K4_OK;
     {
         const SrRows rr = sr_rows(ky0, ky1, 3 + 5 * nrdb + 5, h);          // every SFT layer inside the window reads it
-        SR_DO(run_condnet(n, d_cond, h, w, rr.lo, rr.hi, cond32, fuse ? cond16 : nullptr, s));
+        SR_DO(run_condnet(n, d_cond, h, w, rr.lo, rr.hi, cond32, fuse ? cond16 : nullptr, s), K4_SR_STEP_CONDNET, -1, -1, -1, 0);
     }
     ConvParams c0{};
     c0.H = h; c0.W = w;
@@ -1689,7 +1699,7 @@ static int srnet_forward_roi_impl(const k4_srnet* n, const float* d_x, const flo
             ConvParams p = c0; p.src = in16; p.src_cstride = 32; p.src_c0 = 0; p.mode = SRM_TRUNK_SFT; p.scale = 1.f;
             p.dst_f = feat; p.dst_f2 = tA; p.cond16 = cond16; p.sftw = sft_of(0).frag; p.sft_n = 64; next_dst(p, 0);
             rows(p, 3 + 5 * nrdb);
-            SR_DO(run_conv(n->conv_first, p, s));
+            SR_DO(run_conv(n->conv_first, p, s), K4_SR_STEP_CONV_FIRST, -1, -1, -1, 1);
         }
         for (int i = 0; i < n->num_block; ++i) {
             const float* cur = tA;
@@ -1701,7 +1711,7 @@ static int srnet_forward_roi_impl(const k4_srnet* n, const float* d_x, const flo
                     p.dst_h = cc; p.dst_cstride = 192; p.dst_c0 = 64 + 32 * c;
                     if (c == 3) { p.mode = SRM_STORE_F16_SFT; p.cond16 = cond16; p.sftw = n->rdb_sft[i][j][1].frag; p.sft_n = 32; }
                     rows(p, base + 4 - c);
-                    SR_DO(run_conv(n->rdb_conv[i][j][c], p, s));
+                    SR_DO(run_conv(n->rdb_conv[i][j][c], p, s), K4_SR_STEP_RDB_CONV, i, j, c, c == 3);
                 }
                 {   // x = conv5(cat) * 0.2 + x, then the SFT layer(s) that read it
                     ConvParams p = c0; p.src = cc; p.src_cstride = 192; p.src_c0 = 0; p.scale = 0.2f; p.add_f = cur;
@@ -1714,7 +1724,7 @@ static int srnet_forward_roi_impl(const k4_srnet* n, const float* d_x, const flo
                     }
                     next_dst(p, r + 1);
                     rows(p, base);
-                    SR_DO(run_conv(n->rdb_conv[i][j][4], p, s));
+                    SR_DO(run_conv(n->rdb_conv[i][j][4], p, s), K4_SR_STEP_RDB_CONV, i, j, 4, 1);
                     cur = tB;
                 }
             }
@@ -1722,13 +1732,13 @@ static int srnet_forward_roi_impl(const k4_srnet* n, const float* d_x, const flo
         {   // body_feat = conv_body(sftbody(trunk)) + feat   (sbody was written by the last conv5)
             ConvParams p = c0; p.src = sbody; p.src_cstride = 64; p.mode = SRM_ADD_STORE_F16; p.add_f = feat; p.dst_h = bf; p.dst_cstride = 64;
             rows(p, 2);
-            SR_DO(run_conv(n->conv_body, p, s));
+            SR_DO(run_conv(n->conv_body, p, s), K4_SR_STEP_CONV_BODY, -1, -1, -1, 0);
         }
     } else {
         {   // feat = conv_first(x): fp32 into `feat` and into trunk A (the initial trunk)
             ConvParams p = c0; p.src = in16; p.src_cstride = 32; p.src_c0 = 0; p.mode = SRM_STORE_F32F16; p.dst_f = feat; p.dst_f2 = tA;
             rows(p, 3 + 5 * nrdb);
-            SR_DO(run_conv(n->conv_first, p, s));
+            SR_DO(run_conv(n->conv_first, p, s), K4_SR_STEP_CONV_FIRST, -1, -1, -1, 0);
         }
         for (int i = 0; i < n->num_block; ++i) {
             // RRDB_SFT.forward: trunk A holds x (kept for the block's tail), RDBs update A -> B -> B -> B
@@ -1739,41 +1749,41 @@ static int srnet_forward_roi_impl(const k4_srnet* n, const float* d_x, const flo
                 {   // xc0 = sft0(x) -> cat[0:64]
                     SftParams sp{}; sp.cond = cond32; sp.x_f = cur; sp.dst_h = cat; sp.dst_cstride = 192; sp.dst_c0 = 0;
                     win(sp, base + 5);
-                    SR_DO(run_sft(n->rdb_sft[i][j][0], sp, s));
+                    SR_DO(run_sft(n->rdb_sft[i][j][0], sp, s), K4_SR_STEP_SFT0, i, j, -1, 0);
                 }
                 for (int c = 0; c < 4; ++c) {   // x{c+1} = lrelu(conv(cat[0:64+32c])) -> cat[64+32c : 96+32c]
                     ConvParams p = c0; p.src = cat; p.src_cstride = 192; p.src_c0 = 0; p.mode = SRM_STORE_F16; p.lrelu = 0.2f;
                     p.dst_h = cat; p.dst_cstride = 192; p.dst_c0 = 64 + 32 * c;
                     rows(p, base + 4 - c);
-                    SR_DO(run_conv(n->rdb_conv[i][j][c], p, s));
+                    SR_DO(run_conv(n->rdb_conv[i][j][c], p, s), K4_SR_STEP_RDB_CONV, i, j, c, 0);
                 }
                 {   // xc1 = sft1(x4) in place: cat[160:192]
                     SftParams sp{}; sp.cond = cond32; sp.x_h = cat; sp.xh_cstride = 192; sp.xh_c0 = 160;
                     sp.dst_h = cat; sp.dst_cstride = 192; sp.dst_c0 = 160;
                     win(sp, base + 1);
-                    SR_DO(run_sft(n->rdb_sft[i][j][1], sp, s));
+                    SR_DO(run_sft(n->rdb_sft[i][j][1], sp, s), K4_SR_STEP_SFT1, i, j, -1, 0);
                 }
                 {   // x = conv5(cat) * 0.2 + x
                     ConvParams p = c0; p.src = cat; p.src_cstride = 192; p.src_c0 = 0; p.mode = SRM_TRUNK; p.scale = 0.2f;
                     p.add_f = cur; p.dst_f = tB;
                     rows(p, base);
-                    SR_DO(run_conv(n->rdb_conv[i][j][4], p, s));
+                    SR_DO(run_conv(n->rdb_conv[i][j][4], p, s), K4_SR_STEP_RDB_CONV, i, j, 4, 0);
                     cur = tB;
                 }
             }
             {   // out = sft0(rdb3 out) * 0.2 + x_in  -> A
                 SftParams sp{}; sp.cond = cond32; sp.x_f = tB; sp.dst_f = tA; sp.res_f = tA; sp.res_scale = 0.2f;
                 win(sp, 3 + 5 * (nrdb - 3 * (i + 1)));
-                SR_DO(run_sft(n->rrdb_sft[i], sp, s));
+                SR_DO(run_sft(n->rrdb_sft[i], sp, s), K4_SR_STEP_SFT_RRDB, i, -1, -1, 0);
             }
         }
         {   // body_feat = conv_body(sftbody(trunk)) + feat
             SftParams sp{}; sp.cond = cond32; sp.x_f = tA; sp.dst_h = sbody; sp.dst_cstride = 64; sp.dst_c0 = 0;
             win(sp, 3);
-            SR_DO(run_sft(n->sftbody, sp, s));
+            SR_DO(run_sft(n->sftbody, sp, s), K4_SR_STEP_SFT_BODY, -1, -1, -1, 0);
             ConvParams p = c0; p.src = sbody; p.src_cstride = 64; p.mode = SRM_ADD_STORE_F16; p.add_f = feat; p.dst_h = bf; p.dst_cstride = 64;
             rows(p, 2);
-            SR_DO(run_conv(n->conv_body, p, s));
+            SR_DO(run_conv(n->conv_body, p, s), K4_SR_STEP_CONV_BODY, -1, -1, -1, 0);
         }
     }
     {   // x4: upsample x2 (nearest) + conv + lrelu, twice; then conv_hr + lrelu and conv_last at the output resolution
@@ -1784,22 +1794,22 @@ static int srnet_forward_roi_impl(const k4_srnet* n, const float* d_x, const flo
             p.upsample = 1; p.dst_h = up1;
             p.H = h; p.W = w;                                   // iterate over the SOURCE grid, write the 2x grid
             p.y_lo = clip(ky0 - 1, h); p.y_hi = clip(ky1 + 1, h);                    // -> up1 rows [2ky0-2, 2ky1+2)
-            SR_DO(run_conv_up2x(n->conv_up1, p, s));
+            SR_DO(run_conv_up2x(n->conv_up1, p, s), K4_SR_STEP_UP1, -1, -1, -1, 0);
             p.H = 2 * h; p.W = 2 * w; p.src = up1; p.dst_h = up2;
             p.y_lo = clip(2 * ky0 - 1, 2 * h); p.y_hi = clip(2 * ky1 + 1, 2 * h);    // -> up2 rows [4ky0-2, 4ky1+2)
-            SR_DO(run_conv_up2x(n->conv_up2, p, s));
+            SR_DO(run_conv_up2x(n->conv_up2, p, s), K4_SR_STEP_UP2, -1, -1, -1, 0);
             p.upsample = 0; p.src = up2;
         }
         p.H = sc * h; p.W = sc * w; p.dst_h = hr;
         p.y_lo = clip(sc * ky0 - 1, sc * h); p.y_hi = clip(sc * ky1 + 1, sc * h);
-        SR_DO(run_conv(n->conv_hr, p, s));
+        SR_DO(run_conv(n->conv_hr, p, s), K4_SR_STEP_HR, -1, -1, -1, 0);
         ConvParams q = c0; q.H = sc * h; q.W = sc * w; q.src = hr; q.src_cstride = 64; q.mode = SRM_OUT_NCHW; q.out_nchw = d_out; q.n_valid = 3;
         q.y_lo = sc * ky0; q.y_hi = sc * ky1;
         q.out_ps = out_plane_stride; q.out_rs = out_row_stride;
         q.crop_y0 = sc * ky0; q.crop_y1 = sc * ky1; q.crop_x0 = sc * keep_x0; q.crop_x1 = sc * keep_x1;
         q.n_out_extra = n_extra;
         for (int e = 0; e < n_extra; ++e) q.out_extra[e] = h_extra[e];
-        SR_DO(run_conv(n->conv_last, q, s));
+        SR_DO(run_conv(n->conv_last, q, s), K4_SR_STEP_LAST, -1, -1, -1, 0);
     }
 #undef SR_DO
     return K4_OK;
@@ -1827,6 +1837,26 @@ extern "C" int k4_srnet_forward(const k4_srnet* n, const float* d_x, const float
     if (!n) return K4_ERR_INVALID_ARG;
     const int64_t sc = n->scale;
     return k4_srnet_forward_roi(n, d_x, d_cond, h, w, 0, h, 0, w, d_out, sc * sc * h * w, sc * w, d_ws, ws_bytes, stream);
+}
+
+// The real forward, stopped after `stop_after` steps, for the test suite: the intermediate buffers stay in the workspace.
+extern "C" int k4_testing_srnet_forward_upto(const k4_srnet* n, const float* d_x, const float* d_cond, int32_t h, int32_t w,
+                                             int32_t keep_y0, int32_t keep_y1, int32_t keep_x0, int32_t keep_x1,
+                                             float* d_out, int64_t out_plane_stride, int64_t out_row_stride,
+                                             void* d_ws, size_t ws_bytes, int32_t stop_after,
+                                             k4_sr_step* steps, int32_t max_steps, int32_t* n_steps, k4_sr_ws_layout* ws,
+                                             k4_stream_t stream) {
+    if (n_steps) *n_steps = 0;
+    if (!n || !n_steps || !ws || stop_after < 1 || max_steps < 0 || (max_steps > 0 && !steps)) return K4_ERR_INVALID_ARG;
+    if (h <= 0 || w <= 0) return K4_ERR_INVALID_ARG;
+    const SrWs L = sr_ws(h, w, n->scale);
+    *ws = k4_sr_ws_layout{L.in16, L.cond32, L.cond16, L.feat, L.trunkA, L.trunkB, L.cat, L.cat2, L.sbody, L.bf, L.up1, L.up2,
+                          L.hr, L.total};
+    SrTrace tr{stop_after, max_steps, 0, steps};
+    const int st = srnet_forward_roi_impl(n, d_x, d_cond, h, w, keep_y0, keep_y1, keep_x0, keep_x1, d_out, out_plane_stride,
+                                          out_row_stride, 0, nullptr, d_ws, ws_bytes, stream, &tr);
+    *n_steps = tr.n;
+    return st;
 }
 
 // One decoder layer for the test suite: a throw-away k4_srnet holds the packs (make_conv & co., as k4_srnet_create

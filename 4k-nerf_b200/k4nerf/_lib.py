@@ -106,6 +106,20 @@ class SftTestArgs(C.Structure):
     ]
 
 
+# k4_testing_srnet_forward_upto: the decoder forward's steps (K4_SR_STEP_*) and the workspace layout of a tile
+SR_STEP_KINDS = ('input', 'condnet', 'conv_first', 'rdb_conv', 'sft0', 'sft1', 'sft_rrdb', 'sft_body', 'conv_body', 'up1',
+                 'up2', 'hr', 'last')
+
+
+class SrStep(C.Structure):
+    _fields_ = [('kind', C.c_int32), ('block', C.c_int32), ('dense', C.c_int32), ('conv', C.c_int32), ('fused', C.c_int32)]
+
+
+class SrWsLayout(C.Structure):
+    _fields_ = [(k, C.c_uint64) for k in ('in16', 'cond32', 'cond16', 'feat', 'trunk_a', 'trunk_b', 'cat', 'cat2', 'sbody',
+                                           'bf', 'up1', 'up2', 'hr', 'total')]
+
+
 # k4_testing_march_phases: counters per warpgroup and their slots (marchers: K4_PH_M_*, MLP groups: K4_PH_L_*)
 K4_PHASE_SLOTS = 8
 MARCHER_PHASES = {1: 'setup', 2: 'march', 3: 'rendezvous', 4: 'wait_done', 5: 'drain', 6: 'store'}
@@ -189,6 +203,10 @@ EXPORTS = {
     'k4_testing_conv3x3': (C.c_int, [C.POINTER(ConvTestArgs), C.POINTER(C.c_int32), C.c_void_p]),
     'k4_testing_condnet': (C.c_int, [C.POINTER(CondnetTestArgs), C.POINTER(C.c_int32), C.c_void_p]),
     'k4_testing_sft': (C.c_int, [C.POINTER(SftTestArgs), C.POINTER(C.c_int32), C.c_void_p]),
+    'k4_testing_srnet_forward_upto': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_size_t,
+                                                C.c_int32, C.POINTER(SrStep), C.c_int32, C.POINTER(C.c_int32),
+                                                C.POINTER(SrWsLayout), C.c_void_p]),
     'k4_testing_rgbnet': (C.c_int, [C.c_void_p, C.POINTER(RgbnetTestArgs), C.POINTER(C.c_int32), C.c_void_p]),
     'k4_testing_march_phases': (C.c_int, [C.c_void_p, C.POINTER(RenderArgs), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                           C.POINTER(RenderOut), C.c_void_p, C.c_size_t, C.c_void_p, C.c_int32,

@@ -523,6 +523,48 @@ typedef struct k4_sft_test_args {
 K4_API int k4_testing_sft(const k4_sft_test_args* args, int32_t* kernel_used, k4_stream_t stream);
 
 /*
+ * k4_testing_srnet_forward_upto: k4_srnet_forward_roi (same arguments, same code) that returns after its first
+ * `stop_after` steps, so that a test can read the workspace as the real forward left it after any layer.  A step is one
+ * layer as the forward enqueues it: the NCHW -> NHWC input conversion, CondNet, one convolution (with the SFT layers
+ * fused into its epilogue, if any; conv_up1 / conv_up2 are one step of four phase launches each) or one standalone SFT
+ * pass.  The steps that ran are enqueued on `stream` (not synchronised), exactly as the full forward enqueues them.
+ *   steps[0 .. min(*n_steps, max_steps)) receive the descriptors of the steps that ran, in order; *n_steps their count
+ *   (stop_after, or all steps when stop_after is larger).  *ws receives the byte offsets of the workspace buffers of
+ *   an h x w tile of `net` (the layout every k4_srnet_forward* call uses).
+ *   Arguments are checked before any CUDA call (K4_ERR_INVALID_ARG, *n_steps 0).
+ */
+enum { K4_SR_STEP_INPUT = 0,               /* in16 = fp16 NHWC32 of d_x                          */
+       K4_SR_STEP_CONDNET = 1,             /* cond32 (and cond16 when SFT is fused)              */
+       K4_SR_STEP_CONV_FIRST = 2,
+       K4_SR_STEP_RDB_CONV = 3,            /* conv `conv` (0..4) of dense block `dense` of RRDB `block` */
+       K4_SR_STEP_SFT0 = 4,                /* standalone SFT passes: sft0 / sft1 of a dense block, */
+       K4_SR_STEP_SFT1 = 5,
+       K4_SR_STEP_SFT_RRDB = 6,            /*   the RRDB tail's sft0 (with its residual),        */
+       K4_SR_STEP_SFT_BODY = 7,            /*   sftbody                                          */
+       K4_SR_STEP_CONV_BODY = 8,
+       K4_SR_STEP_UP1 = 9,
+       K4_SR_STEP_UP2 = 10,
+       K4_SR_STEP_HR = 11,
+       K4_SR_STEP_LAST = 12 };
+
+typedef struct k4_sr_step {
+    int32_t kind;                          /* K4_SR_STEP_*                                       */
+    int32_t block, dense, conv;            /* RRDB, dense block in it, conv in that (-1: none)   */
+    int32_t fused;                         /* 1: SFT layer(s) applied in this convolution's epilogue */
+} k4_sr_step;
+
+typedef struct k4_sr_ws_layout {
+    uint64_t in16, cond32, cond16, feat, trunk_a, trunk_b, cat, cat2, sbody, bf, up1, up2, hr, total;   /* byte offsets */
+} k4_sr_ws_layout;
+
+K4_API int k4_testing_srnet_forward_upto(const k4_srnet* net, const float* d_x, const float* d_cond, int32_t h, int32_t w,
+                                         int32_t keep_y0, int32_t keep_y1, int32_t keep_x0, int32_t keep_x1,
+                                         float* d_out, int64_t out_plane_stride, int64_t out_row_stride,
+                                         void* d_workspace, size_t workspace_bytes, int32_t stop_after,
+                                         k4_sr_step* steps, int32_t max_steps, int32_t* n_steps, k4_sr_ws_layout* ws,
+                                         k4_stream_t stream);
+
+/*
  * k4_testing_rgbnet: the scene's packed rgbnet on rows the caller supplies, run by the marchers' own device code for one
  * K4_MLP_* mode, so that a test can compare the colour MLP sample by sample with a reference.
  *   d_x [n][dim0]: model-layout MLP inputs, the vectors the reference's rgbnet receives (rgb_feat: the k0 channels fed to

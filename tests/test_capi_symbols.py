@@ -219,3 +219,37 @@ def test_testing_skip_field_validates_arguments_without_a_gpu():
     cd[:] = [7, 7, 7]
     assert lib.k4_testing_skip_field(C.addressof(scene), C.addressof(buf), 64, cd) == -2
     assert list(cd) == [0, 0, 0]
+
+
+def test_testing_srnet_forward_upto_validates_arguments_without_a_gpu():
+    """k4_testing_srnet_forward_upto (the decoder forward stopped after k steps, for the GPU tests): bad arguments are
+    reported as K4_ERR_INVALID_ARG before any CUDA call, with *n_steps 0.  The net here is a zero-filled host block; every
+    case has an invalid argument, so nothing reads it."""
+    from k4nerf import _lib
+    C = ctypes
+    lib = _lib.lib
+    assert C.sizeof(_lib.SrStep) == 20 and _lib.SrStep.fused.offset == 16                     # the header's layout
+    assert C.sizeof(_lib.SrWsLayout) == 14 * 8 and _lib.SrWsLayout.cond16.offset == 16 and _lib.SrWsLayout.hr.offset == 96
+    assert _lib.SR_STEP_KINDS.index('last') == 12 and _lib.SR_STEP_KINDS.index('sft_rrdb') == 6
+    buf = C.create_string_buffer(64)
+    net = C.create_string_buffer(1 << 16)
+    steps = (_lib.SrStep * 4)()
+    ns = C.c_int32(7)
+    lay = _lib.SrWsLayout()
+
+    def call(**kw):
+        a = dict(net=C.addressof(net), x=C.addressof(buf), cond=C.addressof(buf), h=8, w=8, keep=(0, 8, 0, 8),
+                 out=C.addressof(buf), ws=C.addressof(buf), ws_bytes=64, stop_after=1, steps=steps, max_steps=4,
+                 n_steps=C.byref(ns), layout=C.byref(lay))
+        a.update(kw)
+        ns.value = 7
+        return lib.k4_testing_srnet_forward_upto(a['net'], a['x'], a['cond'], a['h'], a['w'], *a['keep'], a['out'], 64, 8,
+                                                 a['ws'], a['ws_bytes'], a['stop_after'], a['steps'], a['max_steps'],
+                                                 a['n_steps'], a['layout'], None)
+
+    bad = [dict(net=None), dict(stop_after=0), dict(stop_after=-1), dict(max_steps=-1), dict(steps=None),
+           dict(layout=None), dict(h=0), dict(w=-2), dict(net=None, x=None)]
+    for kw in bad:
+        assert call(**kw) == -1, kw
+        assert ns.value == 0, kw
+    assert call(n_steps=None) == -1
