@@ -135,4 +135,17 @@ def true_logit_bound(mode, m, x, diff, D0=None):
     return lg, E
 
 
+def types_ns(st):
+    """The rgbnet shape of an oracle scene as shape_info describes it, with its layers in float64.  The configuration is
+    the one of WS_CFGS with the scene's exact shape."""
+    import types
+    kind = {'dvgo': 'cfgA', 'dmpigo': 'cfgB', 'dcvgo': 'cfgC'}[st['kind']]
+    key = (kind, st['k0_dim'], len(st['viewfreq']), len(st.get('posfreq', [])), st['rgbnet'][0][0].shape[0],
+           int(st.get('rgbnet_direct', True)))
+    cid = next(x[0] for x in WS_CFGS if x[1:] == key)
+    o = shape_info(types.SimpleNamespace(), ('geo', *key, cid))
+    o.layers = [(a.double().numpy(), b.double().numpy()) for a, b in st['rgbnet']]
+    return o
+
+
 FEAT_REL = 2.0 ** -16      # GPU sample inputs against the oracle's (trilinear k0, sin / cos): far below this, relative

@@ -41,7 +41,7 @@ import torch.nn.functional as F
 
 from oracle import ops, pipeline, scenes
 from helpers import model_from_state
-from march_bounds import FEAT_REL, SIG_REL, U, shape_info, sig, true_logit_bound
+from march_bounds import FEAT_REL, SIG_REL, U, sig, true_logit_bound, types_ns
 
 pytestmark = pytest.mark.gpu
 
@@ -410,20 +410,6 @@ def N_samples_of(st, kw):
     return int((st['max_world_size'] - 1) / kw['stepsize']) + 1
 
 
-def types_ns(st):
-    """The rgbnet shape of a scene as march_bounds.shape_info describes it, with its layers in float64."""
-    import types
-    kind = {'dvgo': 'cfgA', 'dmpigo': 'cfgB', 'dcvgo': 'cfgC'}[st['kind']]
-    w = st['rgbnet'][0][0].shape[0]
-    vpe = len(st['viewfreq'])
-    spe = len(st.get('posfreq', []))
-    direct = int(st.get('rgbnet_direct', True))
-    cid = {('cfgA', 128): 1, ('cfgB', 64): 6, ('cfgC', 128): 10}[(kind, w)]
-    o = shape_info(types.SimpleNamespace(), ('geo', kind, st['k0_dim'], vpe, spe, w, direct, cid))
-    o.layers = [(a.double().numpy(), b.double().numpy()) for a, b in st['rgbnet']]
-    return o
-
-
 def check_values(out, ref64, label, ratios):
     for key, got, want, bnd in (('rgb', out['rgb_marched'].double().numpy(), ref64['rgb'], ref64['B']),
                                 ('depth', out['depth'].double().numpy(), ref64['depth'], ref64['BD']),
@@ -435,10 +421,9 @@ def check_values(out, ref64, label, ratios):
         ratios['fp32 vs fp64 ' + key] = float((err[fin] / bnd[fin]).max()) if fin.any() else 0.0
 
 
-def check_tc_against_fp32(fp, outs, st, trace, ref64, skip_rays, label, ratios):
-    """test_every_mode_against_fp32_per_ray's bound, with the weights bounded by the recomposition's w_hi."""
-    if st['rgbnet'] is None:
-        return
+def tc_bounds(st, trace, ref64, rgb_f, modes):
+    """{mode: [N, 3]}: test_every_mode_against_fp32_per_ray's bound on |rgb_mode - rgb_fp32| per ray, with the weights
+    bounded by the recomposition's w_hi; rgb_f is fp32 mode's colour."""
     shp = types_ns(st)
     x = trace['rgb_feat'].double().numpy()
     diff = None if trace['diffuse'] is None else trace['diffuse'].double().numpy()
@@ -446,24 +431,33 @@ def check_tc_against_fp32(fp, outs, st, trace, ref64, skip_rays, label, ratios):
     l_f, E_f = true_logit_bound('fp32', shp, x, diff, D0)
     w = ref64['w_hi'][ref64['si']][:, None]
     rid = trace['ray_id'].long().numpy()
+    N = rgb_f.shape[0]
+    bounds = {}
+    for mode in modes:
+        l_m, E_m = true_logit_bound(mode, shp, x, diff, D0)
+        Em = np.maximum(E_m, E_f)
+        zc = np.clip(0.0, l_f - Em, l_f + Em)
+        dmax = sig(zc) * (1 - sig(zc))
+        s_hi = sig(l_f + Em)
+        per = w * (dmax * (E_m + E_f) + (2 * SIG_REL + 2 * U) * s_hi)
+        B, H = np.zeros((N, 3)), np.zeros((N, 3))
+        np.add.at(B, rid, per)
+        np.add.at(H, rid, w * s_hi)
+        bounds[mode] = B + 2 * np.maximum(ref64['n_c'][:, None] - 1, 0) * U * H + 2 * U * np.abs(rgb_f)
+    return bounds
+
+
+def check_tc_against_fp32(fp, outs, st, trace, ref64, skip_rays, label, ratios):
+    """test_every_mode_against_fp32_per_ray's bound (tc_bounds)."""
+    if st['rgbnet'] is None:
+        return
     N = fp['rgb_marched'].shape[0]
     keep = np.ones(N, bool)
     keep[list(skip_rays)] = False
     rgb_f = fp['rgb_marched'].double().numpy()
-    bounds = {}
+    bounds = tc_bounds(st, trace, ref64, rgb_f, sorted({'ws' if k[1] == 'auto' else k[1] for k in outs}))
     for k, o in outs.items():
         mode = 'ws' if k[1] == 'auto' else k[1]
-        if mode not in bounds:
-            l_m, E_m = true_logit_bound(mode, shp, x, diff, D0)
-            Em = np.maximum(E_m, E_f)
-            zc = np.clip(0.0, l_f - Em, l_f + Em)
-            dmax = sig(zc) * (1 - sig(zc))
-            s_hi = sig(l_f + Em)
-            per = w * (dmax * (E_m + E_f) + (2 * SIG_REL + 2 * U) * s_hi)
-            B, H = np.zeros((N, 3)), np.zeros((N, 3))
-            np.add.at(B, rid, per)
-            np.add.at(H, rid, w * s_hi)
-            bounds[mode] = B + 2 * np.maximum(ref64['n_c'][:, None] - 1, 0) * U * H + 2 * U * np.abs(rgb_f)
         B = bounds[mode]
         d = np.abs(o['rgb_marched'].double().numpy() - rgb_f)
         ok = d[keep] <= B[keep]
@@ -480,23 +474,7 @@ def run_case(st, ms, rays, kw, label, ref_ops=None):
     trace, stats = {}, {}
     ref = pipeline.forward(st, ro, rd, vd, ops.CpuOps, stats=stats, trace=trace, **kw)
     outs = render_all(ms, ro, rd, vd, kw, hw, modes_of(st))
-    # every mode marches the same arithmetic: geometry, transmittance and depth are identical in every mode, order and
-    # skip setting.  fp32 colours are identical too.  A tensor-core mode computes every sample's colour independently
-    # of its batch, but adds a ray's samples in an order that depends on which samples share a batch (the wgmma kernels
-    # through shared-memory atomics, the mma.sync context per flushed group), and skipping and the tile order change the
-    # batches: across skip settings and orders its colours may differ only by that reassociation (order_bound).
-    base = outs[(True, 'fp32', hw)]
-    for key, o in outs.items():
-        for k in ('ray_stats', 't_minmax', 'alphainv_last', 'depth'):
-            assert torch.equal(o[k], base[k]), (label, key, k)
-        assert torch.equal(o['counters'][:3], base['counters'][:3]), (label, key)
-        ref_o = outs[(True, key[1], hw)]
-        if key[1] == 'fp32':
-            assert torch.equal(o['rgb_marched'], ref_o['rgb_marched']), (label, key)
-        else:
-            d = (o['rgb_marched'].double() - ref_o['rgb_marched'].double()).abs()
-            b = order_bound(ref_o, float(kw['bg']))
-            assert bool((d <= b).all()), (label, key, int((d > b).sum()), float((d / b).max()))
+    base = check_modes_agree(outs, hw, float(kw['bg']), label)
     bad = set(check_geometry(base, ref, trace, st, N, label))
     if ref_ops is not None:
         dev = ms[True].density.grid.device
@@ -518,6 +496,28 @@ def run_case(st, ms, rays, kw, label, ref_ops=None):
           f'largest error/bound: this scene {{{", ".join(f"{k}: {v:.3g}" for k, v in ratios.items())}}}  '
           f'all scenes so far {{{", ".join(f"{k}: {v:.3g}" for k, v in RATIOS.items())}}}')
     return base, ref, trace, bad
+
+
+def check_modes_agree(outs, hw, bg, label):
+    """Every mode marches the same arithmetic: geometry, transmittance and depth are identical in every mode, order and
+    skip setting.  fp32 colours are identical too.  A tensor-core mode computes every sample's colour independently of
+    its batch, but adds a ray's samples in an order that depends on which samples share a batch (the wgmma kernels
+    through shared-memory atomics, the mma.sync context per flushed group), and skipping and the tile order change the
+    batches: across skip settings and orders its colours may differ only by that reassociation (order_bound).  Returns
+    the fp32 render with skipping in the order hw."""
+    base = outs[(True, 'fp32', hw)]
+    for key, o in outs.items():
+        for k in ('ray_stats', 't_minmax', 'alphainv_last', 'depth'):
+            assert torch.equal(o[k], base[k]), (label, key, k)
+        assert torch.equal(o['counters'][:3], base['counters'][:3]), (label, key)
+        ref_o = outs[(True, key[1], hw)]
+        if key[1] == 'fp32':
+            assert torch.equal(o['rgb_marched'], ref_o['rgb_marched']), (label, key)
+        else:
+            d = (o['rgb_marched'].double() - ref_o['rgb_marched'].double()).abs()
+            b = order_bound(ref_o, bg)
+            assert bool((d <= b).all()), (label, key, int((d > b).sum()), float((d / b).max()))
+    return base
 
 
 def order_bound(out, bg):
