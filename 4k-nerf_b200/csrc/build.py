@@ -11,7 +11,8 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(os.path.dirname(HERE), 'k4nerf', 'libk4nerf.so')
-SOURCES = ['k4_capi.cu', 'k4_march.cu', 'k4_march_tc.cu', 'k4_march_ws.cu', 'k4_sr.cu', 'k4_ops.cu', 'k4_train.cu', 'k4_distloss.cu']
+SOURCES = ['k4_capi.cu', 'k4_march.cu', 'k4_march_tc.cu', 'k4_march_ws.cu', 'k4_sr.cu', 'k4_ops.cu', 'k4_train.cu', 'k4_distloss.cu',
+           'k4_metrics.cu']
 HEADERS = ['k4_internal.cuh', 'k4_march_common.cuh', 'k4_march_ray.cuh', 'k4_march_ring.cuh', 'k4_march_mma.cuh', 'k4_march_mlp.cuh',
            'k4_ptx.cuh', 'k4_wgmma.cuh', 'k4_ws_cfgs.h',
            '../../include/k4nerf.h']

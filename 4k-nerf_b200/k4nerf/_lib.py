@@ -196,6 +196,10 @@ EXPORTS = {
                                           C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     'k4_op_segment_cumsum': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    'k4_op_rgb_ssim_workspace_bytes': (C.c_size_t, [C.c_int64, C.c_int64, C.c_int32]),
+    'k4_op_rgb_ssim': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.POINTER(C.c_int64),
+                                 C.POINTER(C.c_int64), C.POINTER(C.c_double), C.c_int32, C.c_double, C.c_double, C.c_void_p,
+                                 C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     'k4_make_rays_rows':(C.c_int, [C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_int32,
                                     C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'k4_make_rays': (C.c_int, [C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_int32,

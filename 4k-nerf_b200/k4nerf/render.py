@@ -2,8 +2,8 @@
 
 Differences that do not change results: rays are generated on the device (k4_make_rays), the whole
 frame is ONE fused launch instead of 8192-ray chunks (the chunk loop only bounds the reference's
-intermediate memory, run_sr.py:121-124), and metrics that need packages absent from this image
-(SSIM via scipy is fine, LPIPS is not) raise if requested.
+intermediate memory, run_sr.py:121-124), SSIM is computed on the device (utils.rgb_ssim of CUDA tensors), and
+LPIPS, which needs pretrained weights this project does not ship, raises if requested.
 """
 import numpy as np
 import torch
@@ -67,6 +67,12 @@ def _write_png(filename, rgb8):
     cv2.imwrite(filename, rgb8[..., ::-1])
 
 
+def _ssim_on_device(rgb, gt):
+    """``rgb_ssim(rgb, gt, max_val=1)`` of a clamped frame still on the device (run.py:134-135): the ground truth is
+    uploaded, the frame is not copied back for it."""
+    return rgb_ssim(rgb, torch.as_tensor(gt, device=rgb.device), max_val=1)
+
+
 def _report(psnrs, ssims):
     """run.py:141-145 / run_sr.py:153-157."""
     if len(psnrs):
@@ -95,7 +101,7 @@ def render_viewpoints(model, render_poses, HW, Ks, ndc, render_kwargs,
 
     The reference reads ``cfg.data.flip_x/flip_y`` from a module global (run.py:96); here they come
     from ``render_kwargs`` unless passed explicitly.  The reference's defaults evaluate SSIM and LPIPS-VGG when ground
-    truth is given (here both default to off): ``eval_ssim`` is provided (``utils.rgb_ssim``, CPU), LPIPS needs the
+    truth is given (here both default to off): ``eval_ssim`` scores the frame on the GPU (``utils.rgb_ssim``), LPIPS needs the
     ``lpips`` package and its pretrained VGG / AlexNet weights and raises."""
     assert len(render_poses) == len(HW) and len(HW) == len(Ks)
     if eval_lpips_alex or eval_lpips_vgg:
@@ -107,14 +113,15 @@ def render_viewpoints(model, render_poses, HW, Ks, ndc, render_kwargs,
     frames = _render_frames(model, render_poses, HW, Ks, ndc, render_kwargs, render_factor, flip_x, flip_y)
     rgbs, depths, bgmaps, psnrs, ssims = [], [], [], [], []
     for i, f in enumerate(frames):
-        rgb = f['rgb_marched'].clamp(0, 1).cpu().numpy()
+        rgb_d = f['rgb_marched'].clamp(0, 1)
+        rgb = rgb_d.cpu().numpy()
         rgbs.append(rgb)
         depths.append(f['depth'].cpu().numpy() if f['depth'] is not None else None)
         bgmaps.append(f['alphainv_last'].cpu().numpy())
         if gt_imgs is not None and render_factor == 0:
             psnrs.append(-10. * np.log10(np.mean(np.square(rgb - gt_imgs[i]))))
             if eval_ssim:
-                ssims.append(rgb_ssim(rgb, gt_imgs[i], max_val=1))          # run.py:134-135
+                ssims.append(_ssim_on_device(rgb_d, gt_imgs[i]))          # run.py:134-135
     _report(psnrs, ssims)
     _post(rgbs, depths, bgmaps, render_video_flipy, render_video_rot90)
     _dump(rgbs, savedir, dump_images, global_step)
@@ -139,7 +146,8 @@ def render_viewpoints_sr(model, render_poses, HW, Ks, ndc, render_kwargs,
         raise NotImplementedError('LPIPS evaluation needs the lpips package and its pretrained weights')
     rgbs, rgb_features, depths, bgmaps, psnrs, ssims, viewdirs_all = [], [], [], [], [], [], []
     for i, f in enumerate(frames):
-        rgb = f['rgb_marched'].clamp(0, 1).cpu().numpy()
+        rgb_d = f['rgb_marched'].clamp(0, 1)
+        rgb = rgb_d.cpu().numpy()
         rgbs.append(rgb)
         rgb_features.append(f['rgb_feature'].cpu().numpy())
         depths.append(f['depth'].cpu().numpy())
@@ -148,7 +156,7 @@ def render_viewpoints_sr(model, render_poses, HW, Ks, ndc, render_kwargs,
         if gt_imgs is not None and render_factor == 0:
             psnrs.append(-10. * np.log10(np.mean(np.square(rgb - gt_imgs[i]))))
             if eval_ssim:
-                ssims.append(rgb_ssim(rgb, gt_imgs[i], max_val=1))          # run_sr.py:146-147 (printed, not returned)
+                ssims.append(_ssim_on_device(rgb_d, gt_imgs[i]))          # run_sr.py:146-147 (printed, not returned)
     _report(psnrs, ssims)
     _post(rgbs, depths, bgmaps, render_video_flipy, render_video_rot90)
     _dump(rgbs, savedir, dump_images, global_step)

@@ -400,6 +400,33 @@ K4_API int k4_op_segment_cumsum(const float* d_w, const float* d_s, const int64_
                                 size_t workspace_bytes, k4_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Evaluation metrics (csrc/k4_metrics.cu).
+ *
+ * Replaces: utils.rgb_ssim (lib/utils.py:88-134), the SSIM that render_viewpoints scores frames with (eval_ssim).
+ * d_img0, d_img1: two H x W x 3 images of `dtype` (K4_DTYPE_F32 or K4_DTYPE_F64, both the same), element (y, x, c) at
+ * y * strides[0] + x * strides[1] + c * strides[2] (host arrays of element strides; any value, 0 included, so permuted,
+ * cropped and expanded views are read in place).  h_win: HOST array of the filter_size window taps, c1 = (k1 max_val)^2,
+ * c2 = (k2 max_val)^2, as utils.rgb_ssim computes them.  Per channel, a separable 'valid' blur with the reversed taps
+ * along rows, then columns, gives the means m0 / m1, variances v0 / v1 (clipped at 0) and covariance cov (clipped to
+ * sign(cov) min(sqrt(v0 v1), |cov|)) of every window; the map value is
+ *   ((2 m0 m1 + c1)(2 cov + c2)) / ((m0^2 + m1^2 + c1)(v0 + v1 + c2)).
+ * Every operation is in fp64.  d_map (may be NULL): fp64 [H-f+1, W-f+1, 3] contiguous; d_mean: one device double, the
+ * map's mean.  The workspace holds k4_op_rgb_ssim_workspace_bytes(H, W, filter_size) bytes (0 for an invalid shape),
+ * 8-byte aligned; the mean is summed from per-tile sums in an order fixed by (H, W, filter_size), so it is bitwise
+ * reproducible.  Caller's stream, no host sync.
+ * A NULL pointer (other than d_map), filter_size outside 1 .. K4_SSIM_MAX_FILTER, H or W below filter_size, or another
+ * dtype: K4_ERR_INVALID_ARG; a workspace smaller than the size: K4_ERR_WORKSPACE.
+ */
+#define K4_SSIM_MAX_FILTER 31
+enum { K4_DTYPE_F32 = 0, K4_DTYPE_F64 = 1 };
+/* Replaces: utils.rgb_ssim (lib/utils.py:88-134) -- the workspace of k4_op_rgb_ssim. */
+K4_API size_t k4_op_rgb_ssim_workspace_bytes(int64_t H, int64_t W, int32_t filter_size);
+/* Replaces: utils.rgb_ssim (lib/utils.py:88-134). */
+K4_API int k4_op_rgb_ssim(const void* d_img0, const void* d_img1, int32_t dtype, int64_t H, int64_t W, const int64_t strides0[3],
+                          const int64_t strides1[3], const double* h_win, int32_t filter_size, double c1, double c2,
+                          double* d_map, double* d_mean, void* d_workspace, size_t workspace_bytes, k4_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Testing.  Entry points for the test suite, not for renderers: they replace no reference interface and may change
  * with the kernels they expose.
  *
