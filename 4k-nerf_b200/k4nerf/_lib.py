@@ -200,6 +200,15 @@ EXPORTS = {
     'k4_op_rgb_ssim': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.POINTER(C.c_int64),
                                  C.POINTER(C.c_int64), C.POINTER(C.c_double), C.c_int32, C.c_double, C.c_double, C.c_void_p,
                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    'k4_op_masked_quantiles_workspace_bytes': (C.c_size_t, [C.c_int64, C.c_int64, C.c_int64]),
+    'k4_op_masked_quantiles': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.POINTER(C.c_int64),
+                                         C.POINTER(C.c_int64), C.POINTER(C.c_double), C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_size_t, C.c_void_p]),
+    'k4_op_depth_video_u8': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.POINTER(C.c_int64),
+                                       C.POINTER(C.c_int64), C.c_void_p, C.POINTER(C.c_uint8), C.c_int32, C.c_int32,
+                                       C.c_void_p, C.c_void_p]),
+    'k4_op_frame_u8': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.POINTER(C.c_int64), C.c_int32, C.c_int32, C.c_void_p,
+                                 C.c_void_p]),
     'k4_make_rays_rows':(C.c_int, [C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_int32,
                                     C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'k4_make_rays': (C.c_int, [C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_int32,

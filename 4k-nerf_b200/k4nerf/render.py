@@ -194,6 +194,58 @@ def render_frame_4k(model, net_sr, H, W, K, c2w, ndc, render_kwargs, test_tile=5
 
 
 @torch.no_grad()
+def render_video_4k(model, net_sr, render_poses, HW, Ks, ndc, render_kwargs, render_factor=0, render_video_flipy=False,
+                    render_video_rot90=0, test_tile=510, flip_x=None, flip_y=None, on_frame=None):
+    """The three videos of run_sr.py --render_video (run_sr.py:1399-1463) as the uint8 arrays it hands to
+    ``imageio.mimwrite``: ``(sr [n, s*H', s*W', 3], lr [n, H', W', 3], depth [n, H', W', 3])``, ``s = net_sr.scale``,
+    the primes meaning after ``render_video_rot90``.  Every frame is :func:`render_frame_4k` (``render_factor``
+    scales ``HW`` and ``Ks`` as ``render_viewpoints`` does); its SR and LR frames are quantised on the device
+    (``utils.frame_u8_cuda``), the SR one copied to the host as uint8, and its depth and bgmap stay on the device until
+    the depth video is made from all of them (``utils.depth_video_frames``).
+
+    ``on_frame(i, sr_u8, lr_u8)`` (optional) receives each frame's uint8 CUDA tensors as soon as they exist, e.g. for a
+    streaming encoder; the SR frames are then not kept and ``sr`` is returned as ``None``.  ``lr_u8`` is a view of the
+    LR video's device buffer: copy it to keep it beyond the call.
+
+    With ``render_video_flipy`` / ``render_video_rot90`` all three streams are flipped and rotated, and the decoder
+    reads the unflipped frame and condition, exactly as without them.  (The reference flips the depths it conditions
+    the decoder on but not the decoder's input image, and leaves its SR video unflipped.)"""
+    from .utils import depth_video_frames, frame_u8_cuda
+    assert len(render_poses) == len(HW) and len(HW) == len(Ks)
+    flip_x = render_kwargs.get('flip_x', False) if flip_x is None else flip_x
+    flip_y = render_kwargs.get('flip_y', False) if flip_y is None else flip_y
+    if render_factor != 0:
+        HW = (np.copy(HW) / render_factor).astype(int)
+        Ks = np.copy(Ks)
+        Ks[:, :2, :3] /= render_factor
+    n = len(render_poses)
+    H, W = int(HW[0][0]), int(HW[0][1])
+    if any((int(h), int(w)) != (H, W) for h, w in HW):
+        raise ValueError('render_video_4k: every frame of a video must have the same size')
+    dev = next(model.parameters()).device
+    k = int(render_video_rot90) % 4
+    rot = lambda h, w: (w, h) if k & 1 else (h, w)
+    s = net_sr.scale
+    depths = torch.empty((n, H, W), dtype=torch.float32, device=dev)
+    bgmaps = torch.empty((n, H, W), dtype=torch.float32, device=dev)
+    lr_u8 = torch.empty((n, *rot(H, W), 3), dtype=torch.uint8, device=dev)
+    sr_host = None if on_frame is not None else np.empty((n, *rot(s * H, s * W), 3), dtype=np.uint8)
+    for i, c2w in enumerate(render_poses):
+        sr, lr = render_frame_4k(model, net_sr, H, W, Ks[i], c2w, ndc, render_kwargs, test_tile=test_tile, flip_x=flip_x,
+                                 flip_y=flip_y)
+        depths[i].copy_(lr['depth'].reshape(H, W))
+        bgmaps[i].copy_(lr['alphainv_last'].reshape(H, W))
+        frame_u8_cuda(lr['rgb_marched'].reshape(H, W, 3), render_video_flipy, k, out=lr_u8[i])
+        sr_u8 = frame_u8_cuda(sr.permute(1, 2, 0), render_video_flipy, k)
+        if on_frame is not None:
+            on_frame(i, sr_u8, lr_u8[i])
+        else:
+            torch.from_numpy(sr_host[i]).copy_(sr_u8)
+    depth_u8 = depth_video_frames(depths, bgmaps, q=(5, 95), render_video_flipy=render_video_flipy, render_video_rot90=k)
+    return sr_host, lr_u8.cpu().numpy(), depth_u8.cpu().numpy()
+
+
+@torch.no_grad()
 def render_frame_4k_sharded(model, net_sr, H, W, K, c2w, ndc, render_kwargs, test_tile=510, out_u8=False,
                             flip_x=False, flip_y=False, group=None):
     """:func:`render_frame_4k` across the ranks of ``group`` (one process per GPU, scene and decoder

@@ -97,3 +97,195 @@ def rgb_ssim(img0, img1, max_val, filter_size=11, filter_sigma=1.5, k1=0.01, k2=
     c1, c2 = (k1 * max_val) ** 2, (k2 * max_val) ** 2
     ssim_map = ((2 * m0 * m1 + c1) * (2 * cov + c2)) / ((m0 * m0 + m1 * m1 + c1) * (v0 + v1 + c2))
     return ssim_map if return_map else float(ssim_map.mean())
+
+
+# ------------------------------------------------------------------------------------------------
+# The depth video of run_sr.py --render_video (run_sr.py:1459-1463)
+# ------------------------------------------------------------------------------------------------
+def rainbow_lut_u8():
+    """``to8b`` of matplotlib's ``rainbow`` colormap table, ``[256, 3]`` uint8.  matplotlib defines ``rainbow`` as a
+    ``LinearSegmentedColormap`` of N = 256 entries sampled at ``np.linspace(0, 1, 256)`` from red ``|2x - 0.5|``, green
+    ``sin(pi x)`` and blue ``cos(pi x / 2)``, each clipped to [0, 1]; the expressions below are its own."""
+    x = np.linspace(0, 1, 256)
+    lut = np.clip(np.stack([np.abs(2 * x - 0.5), np.sin(x * np.pi), np.cos(x * np.pi / 2)], -1), 0, 1)
+    return to8b(lut)
+
+
+def _f32_keys(v):
+    """Order-preserving uint32 keys of float32 values (-0.0 before +0.0, every NaN last)."""
+    u = np.ascontiguousarray(v, dtype=np.float32).view(np.uint32)
+    k = np.where(u & 0x80000000, ~u, u | 0x80000000).astype(np.uint32)
+    k[np.isnan(v)] = 0xffffffff
+    return k
+
+
+def _f32_of_keys(k):
+    return np.where(k & 0x80000000, k & 0x7fffffff, ~k).astype(np.uint32).view(np.float32)
+
+
+def _quantile_fractions(q):
+    """``q / 100`` exactly as ``np.percentile`` computes it for float32 data, for a pair of percentiles."""
+    qf = np.true_divide(np.asarray(q, dtype=np.float64), np.float32(100))
+    if qf.shape != (2,):
+        raise ValueError(f'q must be a pair of percentiles, got {q!r}')
+    if not (np.all(0 <= qf) and np.all(qf <= 1)):
+        raise ValueError('Percentiles must be in the range [0, 100]')
+    return qf
+
+
+def masked_quantiles_np(values, q=(5, 95)):
+    """``np.percentile(values, q)`` (method 'linear') of float32 values, restated from their order statistics as the
+    kernel computes it: sorted order-preserving keys, numpy's indexes (``_get_indexes``: virtual index ``(n - 1) q``,
+    both neighbours the last value at or above the last index, where numpy's previous index is -1 and its gamma
+    ``virtual + 1``) and numpy's ``_lerp`` (the difference in float32, the rest in float64).  Returns two
+    ``np.float64``; NaN among the values gives NaN, as numpy; no values raise ``ValueError``."""
+    qf = _quantile_fractions(q)
+    v = np.asarray(values, dtype=np.float32).ravel()
+    n = v.size
+    if n == 0:
+        raise ValueError('the depth video needs at least one pixel with bgmap < 0.1')
+    s = _f32_of_keys(np.sort(_f32_keys(v)))
+    out = []
+    for t in qf:
+        vi = np.float64(n - 1) * t
+        if vi >= n - 1:
+            prev = nxt = n - 1
+            gamma = vi - np.float64(-1)
+        else:
+            prev = int(np.floor(vi))
+            nxt = prev + 1
+            gamma = vi - np.float64(prev)
+        a, b = s[prev], s[nxt]
+        with np.errstate(invalid='ignore'):                                 # inf - inf, as numpy's own
+            d = np.float64(np.float32(b - a))
+            r = np.float64(b) - d * (1 - gamma) if gamma >= 0.5 else np.float64(a) + d * gamma
+        out.append(np.float64(np.nan) if np.isnan(v).any() else np.float64(r))
+    return out[0], out[1]
+
+
+def _flip_rot(frames, render_video_flipy, render_video_rot90):
+    """``render_video_flipy`` then ``render_video_rot90`` of render.py's ``_post``, on ``[n, H, W, ...]`` frames."""
+    if render_video_flipy:
+        frames = np.flip(frames, axis=1)
+    return np.ascontiguousarray(np.rot90(frames, k=render_video_rot90, axes=(1, 2)))
+
+
+def _frames_of(x, name):
+    """``[n, H, W]`` of an ``[n, H, W]`` or ``[n, H, W, 1]`` array / tensor (a view)."""
+    if x.ndim == 4 and x.shape[-1] == 1:
+        x = x[..., 0]
+    if x.ndim != 3:
+        raise ValueError(f'{name} must be [n, H, W] or [n, H, W, 1], got shape {tuple(x.shape)}')
+    return x
+
+
+def _depth_video_np(depths, bgmaps, q, render_video_flipy, render_video_rot90):
+    """run_sr.py:1459-1463 in numpy, the colormap restated (``rainbow_lut_u8``) and the percentiles by
+    ``masked_quantiles_np``; ``Colormap.__call__``'s index: trunc(256 x), 256 -> 255, NaN -> the 'bad' colour."""
+    depths = _frames_of(np.asarray(depths, dtype=np.float32), 'depths')
+    bgmaps = _frames_of(np.asarray(bgmaps, dtype=np.float32), 'bgmaps')
+    if depths.shape != bgmaps.shape:
+        raise ValueError(f'depths {depths.shape} and bgmaps {bgmaps.shape} differ')
+    depths_vis = depths * (1 - bgmaps) + bgmaps
+    dmin, dmax = masked_quantiles_np(depths_vis[bgmaps < 0.1], q)
+    with np.errstate(divide='ignore', invalid='ignore'):
+        x = 1 - np.clip((depths_vis - dmin) / (dmax - dmin), 0, 1)
+        xa = x * 256
+        xa[xa == 256] = 255
+        bad = np.isnan(xa)
+        idx = xa.astype(int)
+    idx[bad] = 0
+    frames = rainbow_lut_u8()[idx]
+    frames[bad] = 0
+    return _flip_rot(frames, render_video_flipy, render_video_rot90), dmin, dmax
+
+
+def _strides3(t):
+    import ctypes as C
+    return (C.c_int64 * 3)(*t.stride())
+
+
+def _cuda_call(fn, *args):
+    from . import _lib
+    _lib.check(getattr(_lib.lib, fn)(*args), fn)
+
+
+def _depth_video_cuda(depths, bgmaps, q, render_video_flipy, render_video_rot90):
+    """``k4_op_masked_quantiles`` + ``k4_op_depth_video_u8`` (csrc/k4_video.cu) on float32 CUDA tensors, read in place;
+    one 24-byte read of the range and count between them."""
+    import ctypes as C
+    from . import _lib
+    if not (_is_cuda(depths) and _is_cuda(bgmaps) and depths.device == bgmaps.device):
+        raise RuntimeError('depth_video_frames: depths and bgmaps must both be numpy / CPU or both on one CUDA device')
+    if depths.dtype != torch.float32 or bgmaps.dtype != torch.float32:
+        raise TypeError(f'depth_video_frames: float32 depths and bgmaps expected, got {depths.dtype} and {bgmaps.dtype}')
+    depths, bgmaps = _frames_of(depths.detach(), 'depths'), _frames_of(bgmaps.detach(), 'bgmaps')
+    if depths.shape != bgmaps.shape:
+        raise ValueError(f'depths {tuple(depths.shape)} and bgmaps {tuple(bgmaps.shape)} differ')
+    n, H, W = depths.shape
+    qf = _quantile_fractions(q)
+    k = int(render_video_rot90) % 4
+    dev = depths.device
+    with torch.cuda.device(dev):
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        ws = torch.empty(_lib.lib.k4_op_masked_quantiles_workspace_bytes(n, H, W), dtype=torch.uint8, device=dev)
+        res = torch.empty(3, dtype=torch.int64, device=dev)              # dmin, dmax (fp64 bits), count
+        sd, sb = _strides3(depths), _strides3(bgmaps)
+        _cuda_call('k4_op_masked_quantiles', C.c_void_p(depths.data_ptr()), C.c_void_p(bgmaps.data_ptr()), n, H, W, sd, sb,
+                   (C.c_double * 2)(*qf.tolist()), C.c_void_p(res.data_ptr()), C.c_void_p(res.data_ptr() + 16),
+                   C.c_void_p(ws.data_ptr()), ws.numel(), stream)
+        host = res.cpu().numpy()
+        if host[2] == 0:
+            raise ValueError('the depth video needs at least one pixel with bgmap < 0.1')
+        dmin, dmax = host[:2].view(np.float64)
+        out = torch.empty((n, W, H, 3) if k & 1 else (n, H, W, 3), dtype=torch.uint8, device=dev)
+        lut = np.ascontiguousarray(rainbow_lut_u8())
+        _cuda_call('k4_op_depth_video_u8', C.c_void_p(depths.data_ptr()), C.c_void_p(bgmaps.data_ptr()), n, H, W, sd, sb,
+                   C.c_void_p(res.data_ptr()), lut.ctypes.data_as(C.POINTER(C.c_uint8)), int(bool(render_video_flipy)), k,
+                   C.c_void_p(out.data_ptr()), stream)
+    return out, np.float64(dmin), np.float64(dmax)
+
+
+def depth_video_frames(depths, bgmaps, q=(5, 95), render_video_flipy=False, render_video_rot90=0, return_range=False):
+    """The depth video of run_sr.py --render_video (run_sr.py:1459-1463) as uint8 frames ``[n, H', W', 3]``:
+    ``depths_vis = depths * (1 - bgmaps) + bgmaps`` (float32), ``dmin, dmax = np.percentile(depths_vis[bgmaps < 0.1],
+    q)``, then ``to8b`` of matplotlib's ``rainbow`` colormap of ``1 - clip((depths_vis - dmin) / (dmax - dmin), 0, 1)``,
+    flipped (``render_video_flipy``, axis 0 of a frame) and then rotated (``np.rot90`` by ``render_video_rot90``) as
+    ``render_viewpoints`` flips and rotates its outputs.  H' x W' is W x H for an odd rotation.
+
+    ``depths``, ``bgmaps``: ``[n, H, W, 1]`` (as ``render_viewpoints`` returns them) or ``[n, H, W]``, float32.  CUDA
+    tensors run on the GPU (``k4_op_masked_quantiles`` and ``k4_op_depth_video_u8``, any strides) and give a CUDA
+    tensor; numpy arrays and CPU tensors take the numpy restatement and give a numpy array.  Both give numpy's values
+    bit for bit.  ``return_range=True`` also returns ``(dmin, dmax)`` as ``np.float64``.
+
+    Edge cases, all as numpy and matplotlib: with ``dmax == dmin`` a pixel below the range is colour 255 (x = 1),
+    above it colour 0, and on it 0 / 0 = NaN, the colormap's 'bad' colour (0, 0, 0); pixels on dmin / dmax map to
+    x = 1 / 0; ``bgmaps == 0.1`` is not selected; NaN depths give the bad colour, and a NaN among the selected values
+    makes the range NaN.  No selected pixel raises ``ValueError`` (numpy raises ``IndexError`` there).  The reference's
+    ``.squeeze()`` would also drop a frame axis of length 1; here the shape stays ``[n, H', W', 3]``."""
+    if _is_cuda(depths) or _is_cuda(bgmaps):
+        out, dmin, dmax = _depth_video_cuda(depths, bgmaps, q, render_video_flipy, render_video_rot90)
+    else:
+        out, dmin, dmax = _depth_video_np(depths, bgmaps, q, render_video_flipy, render_video_rot90)
+    return (out, (dmin, dmax)) if return_range else out
+
+
+def frame_u8_cuda(rgb, render_video_flipy=False, render_video_rot90=0, out=None):
+    """``to8b`` of one float32 ``[H, W, 3]`` CUDA frame (any strides, e.g. ``sr.permute(1, 2, 0)`` of a decoder
+    output), flipped and rotated like :func:`depth_video_frames`, by ``k4_op_frame_u8``: a uint8 ``[H', W', 3]`` CUDA
+    tensor (written into ``out`` when given, which must be contiguous)."""
+    import ctypes as C
+    if not _is_cuda(rgb) or rgb.dtype != torch.float32 or rgb.ndim != 3 or rgb.shape[-1] != 3:
+        raise ValueError(f'frame_u8_cuda: a float32 [H, W, 3] CUDA tensor expected, got {getattr(rgb, "shape", None)}')
+    H, W = rgb.shape[0], rgb.shape[1]
+    k = int(render_video_rot90) % 4
+    shape = (W, H, 3) if k & 1 else (H, W, 3)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.uint8, device=rgb.device)
+    elif tuple(out.shape) != shape or out.dtype != torch.uint8 or not out.is_contiguous() or out.device != rgb.device:
+        raise ValueError(f'frame_u8_cuda: out must be a contiguous uint8 {shape} tensor on {rgb.device}')
+    rgb = rgb.detach()
+    with torch.cuda.device(rgb.device):
+        _cuda_call('k4_op_frame_u8', C.c_void_p(rgb.data_ptr()), H, W, _strides3(rgb), int(bool(render_video_flipy)), k,
+                   C.c_void_p(out.data_ptr()), C.c_void_p(torch.cuda.current_stream(rgb.device).cuda_stream))
+    return out

@@ -427,6 +427,57 @@ K4_API int k4_op_rgb_ssim(const void* d_img0, const void* d_img1, int32_t dtype,
                           double* d_map, double* d_mean, void* d_workspace, size_t workspace_bytes, k4_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Video streams of run_sr.py --render_video (csrc/k4_video.cu).
+ *
+ * k4_op_masked_quantiles replaces the depth video's range, run_sr.py:1459-1461:
+ *   depths_vis = depths * (1 - bgmaps) + bgmaps;  dmin, dmax = np.percentile(depths_vis[bgmaps < 0.1], q=[5, 95])
+ * d_depth, d_bgmap: n x H x W fp32, element (f, y, x) at f * strides[0] + y * strides[1] + x * strides[2] (host arrays of
+ * element strides, so [n, H, W, 1] arrays and views are read in place).  depths_vis is formed in fp32 with one rounding
+ * per operation, the selection is bgmap < 0.1f.  h_q: HOST array of the two quantiles as fractions, q / 100 as numpy's
+ * percentile computes it (np.true_divide(q, np.float32(100)), fp64), each in [0, 1].  d_quantiles (2 device doubles)
+ * receives np.percentile's 'linear' values bit for bit: the order statistics are exact (a radix select on the fp32
+ * keys: integer counts only) and the interpolation is numpy's _lerp.  A NaN among the selected values gives NaN, as
+ * numpy.  d_count (one device int64) receives the number of selected values; with 0 the quantiles are NaN (numpy
+ * raises).  -0.0 orders before +0.0 (numpy treats them as equal, so a quantile that falls on a tie between them may
+ * carry either sign there).  The workspace holds k4_op_masked_quantiles_workspace_bytes(n, H, W) bytes (0 for an
+ * invalid shape), 16-byte aligned.  Caller's stream, no host sync; the result is bitwise reproducible.
+ * A NULL pointer, n, H or W below 1, n * H above 2^31 - 1, a quantile outside [0, 1] or NaN, or a misaligned pointer:
+ * K4_ERR_INVALID_ARG; a workspace smaller than the size: K4_ERR_WORKSPACE.
+ *
+ * k4_op_depth_video_u8 replaces run_sr.py:1462-1463's frames:
+ *   to8b(plt.get_cmap('rainbow')(1 - np.clip((depths_vis - dmin) / (dmax - dmin), 0, 1)).squeeze()[..., :3])
+ * with render_video_flipy / render_video_rot90 (render.py's _post) applied.  d_range: the two device doubles dmin, dmax
+ * (k4_op_masked_quantiles' d_quantiles).  The normalisation is fp64, as numpy 2 computes float32 - float64.  Colormap
+ * index: i = trunc(256 x), 256 -> 255; NaN x (dmax == dmin at depths_vis == dmin, or NaN data) is the colormap's 'bad'
+ * colour, (0, 0, 0).  h_lut: HOST u8 [256][3], to8b of the colormap's rgb table.  d_out: u8 [n, H', W', 3] contiguous,
+ * H' x W' = H x W for even rot90 and W x H for odd; frame f is rot90(flip(frame f, axis 0) if flip_y, rot90 mod 4).
+ * n, H or W outside 1 .. 65535, flip_y not 0 / 1, a NULL or misaligned pointer: K4_ERR_INVALID_ARG.
+ *
+ * k4_op_frame_u8 replaces utils.to8b (lib/utils.py:20) of one rendered frame, (255 * np.clip(x, 0, 1)).astype(uint8)
+ * with the product in fp32, with the same flip / rot90.  d_rgb: H x W x 3 fp32, element (y, x, c) at y * strides[0] +
+ * x * strides[1] + c * strides[2], e.g. a [3, H, W] decoder output read as permute(1, 2, 0).  NaN gives 0.
+ * d_out: u8 [H', W', 3] contiguous.  H or W outside 1 .. 65535, flip_y not 0 / 1, a NULL or misaligned pointer:
+ * K4_ERR_INVALID_ARG.
+ */
+/* Replaces: np.percentile(depths_vis[bgmaps < 0.1], q=[5, 95]) (run_sr.py:1460) -- the workspace of
+ * k4_op_masked_quantiles. */
+K4_API size_t k4_op_masked_quantiles_workspace_bytes(int64_t n, int64_t H, int64_t W);
+/* Replaces: depths_vis = depths * (1-bgmaps) + bgmaps; np.percentile(depths_vis[bgmaps < 0.1], q=[5, 95])
+ * (run_sr.py:1459-1460). */
+K4_API int k4_op_masked_quantiles(const float* d_depth, const float* d_bgmap, int64_t n, int64_t H, int64_t W,
+                                  const int64_t depth_strides[3], const int64_t bgmap_strides[3], const double h_q[2],
+                                  double* d_quantiles, int64_t* d_count, void* d_workspace, size_t workspace_bytes,
+                                  k4_stream_t stream);
+/* Replaces: to8b(plt.get_cmap('rainbow')(1 - np.clip((depths_vis - dmin) / (dmax - dmin), 0, 1)).squeeze()[..., :3])
+ * (run_sr.py:1461-1463), flipped / rotated as render_viewpoints' render_video_flipy / render_video_rot90. */
+K4_API int k4_op_depth_video_u8(const float* d_depth, const float* d_bgmap, int64_t n, int64_t H, int64_t W,
+                                const int64_t depth_strides[3], const int64_t bgmap_strides[3], const double* d_range,
+                                const uint8_t* h_lut, int32_t flip_y, int32_t rot90, uint8_t* d_out, k4_stream_t stream);
+/* Replaces: utils.to8b (lib/utils.py:20) of the video frames (run_sr.py:1457-1458), flipped / rotated. */
+K4_API int k4_op_frame_u8(const float* d_rgb, int64_t H, int64_t W, const int64_t strides[3], int32_t flip_y, int32_t rot90,
+                          uint8_t* d_out, k4_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Testing.  Entry points for the test suite, not for renderers: they replace no reference interface and may change
  * with the kernels they expose.
  *
