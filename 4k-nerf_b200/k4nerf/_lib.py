@@ -134,6 +134,26 @@ class RgbnetTestArgs(C.Structure):
     ]
 
 
+class TrainMarchArgs(C.Structure):
+    """k4_train_march_args: one fused scene-training step's render and loss (k4_train_march_forward / _backward)."""
+    _fields_ = [
+        ('kind', C.c_int32), ('rgbnet_act', C.c_int32), ('n_rays', C.c_int64), ('world_size', C.c_int32 * 3),
+        ('k0_dim', C.c_int32), ('mask_size', C.c_int32 * 3), ('mpi_depth', C.c_int32),
+        ('xyz_min', C.c_float * 3), ('xyz_max', C.c_float * 3), ('xyz2ijk_scale', C.c_float * 3), ('xyz2ijk_shift', C.c_float * 3),
+        ('act_shift', C.c_float), ('voxel_size', C.c_float), ('interval', C.c_float), ('fast_color_thres', C.c_float),
+        ('near_', C.c_float), ('stepsize', C.c_float), ('bg', C.c_float), ('max_world_size', C.c_int32),
+        ('rgbnet_depth', C.c_int32), ('rgbnet_width', C.c_int32), ('rgbnet_direct', C.c_int32),
+        ('viewbase_pe', C.c_int32), ('spatial_pe', C.c_int32), ('rgbnet_act_param', C.c_float),
+        ('w_main', C.c_float), ('w_entropy', C.c_float), ('w_distortion', C.c_float), ('w_rgbper', C.c_float),
+        ('d_rays_o', C.c_void_p), ('d_rays_d', C.c_void_p), ('d_viewdirs', C.c_void_p), ('d_target', C.c_void_p),
+        ('d_bkgd', C.c_void_p), ('d_density', C.c_void_p), ('d_k0', C.c_void_p), ('d_mask', C.c_void_p),
+        ('d_act_shift_grid', C.c_void_p), ('d_rgbnet_weight', C.c_void_p * 3), ('d_rgbnet_bias', C.c_void_p * 3),
+        ('d_rgb_marched', C.c_void_p), ('d_alphainv_last', C.c_void_p), ('d_loss', C.c_void_p), ('d_loss_terms', C.c_void_p),
+        ('d_grad_density', C.c_void_p), ('d_grad_k0', C.c_void_p), ('d_grad_weight', C.c_void_p * 3),
+        ('d_grad_bias', C.c_void_p * 3),
+    ]
+
+
 EXPORTS = {
     'k4_abi_version': (C.c_int, []),
     'k4_status_string': (C.c_char_p, [C.c_int]),
@@ -225,6 +245,9 @@ EXPORTS = {
                                           C.POINTER(RenderOut), C.c_void_p, C.c_size_t, C.c_void_p, C.c_int32,
                                           C.POINTER(C.c_int32), C.c_void_p]),
     'k4_testing_skip_field': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int32)]),
+    'k4_train_march_workspace_bytes': (C.c_size_t, [C.c_int64]),
+    'k4_train_march_forward': (C.c_int, [C.POINTER(TrainMarchArgs), C.c_void_p, C.c_size_t, C.c_void_p]),
+    'k4_train_march_backward': (C.c_int, [C.POINTER(TrainMarchArgs), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 if not os.path.exists(LIB_PATH):

@@ -399,6 +399,72 @@ K4_API int k4_op_segment_cumsum(const float* d_w, const float* d_s, const int64_
                                 float* d_w_prefix, float* d_w_total, float* d_ws_prefix, float* d_ws_total, void* d_workspace,
                                 size_t workspace_bytes, k4_stream_t stream);
 
+/* One scene-training step's render and loss, fused (csrc/k4_train_march.cu): the training forward of DirectVoxGO /
+ * DirectMPIGO (lib/dvgo.py:327-448, lib/dmpigo.py:292-427) and run_sr.py's composite loss (run_sr.py:521-546, without
+ * nearclip) in one forward kernel, and its gradient in one backward kernel that re-marches every ray.  The parameters are
+ * read live, in their own layouts: density [X,Y,Z] (of [1,1,X,Y,Z]), k0 planar [C,X,Y,Z], mask [mX,mY,mZ] bytes, the MPI
+ * act_shift [mpi_depth], rgbnet weights [out,in] and biases [out].  Loss terms (a weight of 0 skips its term):
+ *   main          w_main * mean((rgb_marched - target)^2)
+ *   entropy_last  w_entropy * mean over rays of the entropy of clamp(alphainv_last, 1e-6, 1 - 1e-6)
+ *   distortion    w_distortion * flatten_eff_distloss(weights, s, 1 / n_samples, ray_id), divided by the largest shaded
+ *                 ray id + 1 (DirectMPIGO only)
+ *   rgbper        w_rgbper * sum over shaded samples of weight * |rgb - target|^2, divided by n_rays
+ * d_loss [1] receives their sum, d_loss_terms [4] each weighted term (0 when skipped); both are bitwise reproducible.
+ * d_bkgd [n_rays,3] (may be NULL: the scalar bg) is the background under rand_bkgd.  The backward ADDS dL/d(parameter),
+ * times the device scalar *d_grad_loss, into the d_grad_* arrays (same layouts as the parameters; a NULL one is not
+ * computed); the caller zero-fills them.  It reads what the forward left in the workspace
+ * (k4_train_march_workspace_bytes(n_rays) bytes, 16-byte aligned).  Caller's stream, no host synchronisation.
+ * A NULL pointer, n_rays < 1 or a bad enum / size: K4_ERR_INVALID_ARG; DirectContractedVoxGO, an rgbnet depth other
+ * than 0 or 3, k0_dim > 32, width > 128, an MLP input wider than 128, a pe above 10: K4_ERR_UNSUPPORTED; both before
+ * any CUDA call. */
+typedef struct k4_train_march_args {
+    int32_t kind;                 /* K4_KIND_DVGO / K4_KIND_DMPIGO                                   */
+    int32_t rgbnet_act;           /* K4_ACT_* of the hidden layers (DirectMPIGO's act_type)          */
+    int64_t n_rays;
+    int32_t world_size[3];        /* density / k0 grid X, Y, Z                                       */
+    int32_t k0_dim;
+    int32_t mask_size[3];
+    int32_t mpi_depth;
+    float xyz_min[3], xyz_max[3];
+    float xyz2ijk_scale[3], xyz2ijk_shift[3];
+    float act_shift;              /* DirectVoxGO                                                     */
+    float voxel_size;             /* DirectVoxGO: stepdist = stepsize * voxel_size (fp32)            */
+    float interval;               /* float(stepsize * voxel_size_ratio), as the training forward     */
+    float fast_color_thres;
+    float near_, stepsize, bg;
+    int32_t max_world_size;
+    int32_t rgbnet_depth;         /* 0 (colour grid) or 3                                            */
+    int32_t rgbnet_width;
+    int32_t rgbnet_direct;
+    int32_t viewbase_pe, spatial_pe;
+    float rgbnet_act_param;       /* K4_ACT_GAUSS: GaussianActivation.a                              */
+    float w_main, w_entropy, w_distortion, w_rgbper;
+    const float* d_rays_o;        /* [n_rays,3] each                                                 */
+    const float* d_rays_d;
+    const float* d_viewdirs;
+    const float* d_target;
+    const float* d_bkgd;
+    const float* d_density;
+    const float* d_k0;
+    const uint8_t* d_mask;
+    const float* d_act_shift_grid;
+    const float* d_rgbnet_weight[3];
+    const float* d_rgbnet_bias[3];
+    float* d_rgb_marched;         /* [n_rays,3]  forward outputs                                     */
+    float* d_alphainv_last;       /* [n_rays]                                                        */
+    float* d_loss;                /* [1]                                                             */
+    float* d_loss_terms;          /* [4]: main, entropy_last, distortion, rgbper                     */
+    float* d_grad_density;        /* backward outputs (accumulated)                                  */
+    float* d_grad_k0;
+    float* d_grad_weight[3];
+    float* d_grad_bias[3];
+} k4_train_march_args;
+
+K4_API size_t k4_train_march_workspace_bytes(int64_t n_rays);
+K4_API int k4_train_march_forward(const k4_train_march_args* args, void* d_workspace, size_t workspace_bytes, k4_stream_t stream);
+K4_API int k4_train_march_backward(const k4_train_march_args* args, const float* d_grad_loss, const void* d_workspace,
+                                   size_t workspace_bytes, k4_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Evaluation metrics (csrc/k4_metrics.cu).
  *
