@@ -142,3 +142,20 @@ int k4_launch_march_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st, u
                        int max_ctas = 0, int* n_ctas = nullptr);
 // k4_testing_rgbnet for the wgmma modes (arguments already checked; k4_capi.cu runs the other modes)
 int k4_testing_rgbnet_ws(const k4_scene* sc, const k4_rgbnet_test_args* a, cudaStream_t st);
+
+// A 3x3 / pad 1 convolution with bias and ReLU on the decoder's wgmma kernels (k4_sr.cu), for LPIPS's VGG16
+// (k4_lpips.cu), with every value carried as an fp16 pair hi = fp16(x), lo = fp16(x - hi).  k4_conv3x3_pack packs
+// w [cout][cin][3][3] and b [cout] (fp32, device) into one allocation: cout / 64 blocks of 64 output channels, K = 3 cin
+// (the weights w_hi, w_hi, w_lo against the activations' hi, lo, hi copies).  k4_conv3x3_relu_split reads src, fp16
+// NHWC with cin_pad channels per pixel ([hi | lo | hi] of cin channels each, then zeros), and writes dst, fp16 NHWC
+// with 3 cout channels: [hi | lo | hi] of max(conv + b, 0) (fp32 accumulation).  Caller's stream, no host sync.
+struct K4Conv3x3Pack {
+    void* blob;
+    unsigned char* wpack;         // [cout / 64][ws_bytes]: conv3x3_ws_kernel packs
+    float* bias;                  // [cout]
+    size_t ws_bytes;
+    int cin, cin_pad, cout;       // cin_pad = 3 cin rounded up to 32
+};
+int k4_conv3x3_pack(const float* w, const float* b, int cout, int cin, cudaStream_t s, K4Conv3x3Pack* c);
+void k4_conv3x3_free(K4Conv3x3Pack* c);
+int k4_conv3x3_relu_split(const K4Conv3x3Pack& c, const __half* src, int H, int W, __half* dst, cudaStream_t s);

@@ -78,6 +78,9 @@ struct ConvParams {
     // (sft_frag_layout), the fp16 destination of the (last) modulated result, the RRDB input for the block tail
     const __half* cond16; const unsigned char* sftw; const unsigned char* sftw2; int sft_n;
     __half* dst_h2; int dst2_cstride, dst2_c0; const float* add_f2; float scale2;
+    // SRM_STORE_F16 with lrelu == 0 (LPIPS's VGG16, k4_conv3x3_relu_split): relu = max(x, 0); split > 0 also stores
+    // lo = fp16(x - hi) at channel + split and hi again at channel + 2 split, the input layout of the next such layer
+    int relu, split;
 };
 
 __device__ __forceinline__ void sr_store_out(const ConvParams& p, long long idx, float v) {
@@ -282,8 +285,8 @@ __device__ __forceinline__ void epilogue_sft(const ConvParams& p, const unsigned
 }
 
 // Epilogue of one 16-pixel block for the plain modes: pixels (py, px) and (py + 1, px) of the iteration grid, channels
-// 8j+2t, +1 of accumulator registers 4j .. 4j+3.
-template <int N>
+// 8j+2t, +1 of accumulator registers 4j .. 4j+3.  SPLIT: the kernel honours ConvParams::split (conv3x3_ws_kernel only).
+template <int N, bool SPLIT>
 __device__ __forceinline__ void epilogue_plain(const ConvParams& p, const float* sbias, const float (&acc)[N / 2], int pyA, int px, int tq) {
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -298,7 +301,15 @@ __device__ __forceinline__ void epilogue_plain(const ConvParams& p, const float*
             float o0 = acc[4 * j + 2 * r] + sbias[ch], o1 = acc[4 * j + 2 * r + 1] + sbias[ch + 1];
             if (p.mode == SRM_STORE_F16) {
                 if (p.lrelu > 0.f) { o0 = o0 > 0.f ? o0 : o0 * p.lrelu; o1 = o1 > 0.f ? o1 : o1 * p.lrelu; }
-                *reinterpret_cast<uint32_t*>(p.dst_h + pix * p.dst_cstride + p.dst_c0 + ch) = h2_sat(o0, o1);
+                else if (p.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
+                __half* d = p.dst_h + pix * p.dst_cstride + p.dst_c0 + ch;
+                const uint32_t hi = h2_sat(o0, o1);
+                *reinterpret_cast<uint32_t*>(d) = hi;
+                if (SPLIT && p.split) {
+                    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+                    *reinterpret_cast<uint32_t*>(d + p.split) = h2_sat(o0 - f.x, o1 - f.y);
+                    *reinterpret_cast<uint32_t*>(d + 2 * p.split) = hi;
+                }
             } else if (p.mode == SRM_TRUNK) {
                 const float2 a = __ldg(reinterpret_cast<const float2*>(p.add_f + pix * 64 + ch));
                 *reinterpret_cast<float2*>(p.dst_f + pix * 64 + ch) = make_float2(o0 * p.scale + a.x, o1 * p.scale + a.y);
@@ -460,7 +471,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) conv3x3_ws_kernel(const __grid_
                     if (p.mode >= SRM_STORE_F16_SFT) {
                         if constexpr (N >= 32) epilogue_sft<N>(p, sftw_s, sbias, acc[ml][mh], pyA, px, lane);
                     } else {
-                        epilogue_plain<N>(p, sbias, acc[ml][mh], pyA, px, tq);
+                        epilogue_plain<N, true>(p, sbias, acc[ml][mh], pyA, px, tq);
                     }
                 }
         }
@@ -576,7 +587,7 @@ __global__ void __launch_bounds__(K64_THREADS, 1) conv3x3_k64_kernel(const __gri
             for (int h = 0; h < 3; ++h) {
                 wg_fence_acc(acc[h]);
                 const int j = 3 * wg + h, m = j >> 1, mh = j & 1;
-                epilogue_plain<N>(p, sbias, acc[h], y0 + 8 * mh + 2 * wq, x0 + 8 * m + g8, tq);
+                epilogue_plain<N, false>(p, sbias, acc[h], y0 + 8 * mh + 2 * wq, x0 + 8 * m + g8, tq);
             }
         }
     }
@@ -1429,7 +1440,7 @@ int run_conv(const SrConv& c, ConvParams p, cudaStream_t s, const __half* wk64_o
     if (p.y_lo < 0) p.y_lo = 0;
     if (p.y_hi > p.H) p.y_hi = p.H;
     if (p.y_hi <= p.y_lo) return K4_OK;
-    const bool k64_ok = wk64 && p.cin == 64 && !p.upsample && (p.src_cstride % 8) == 0 && (p.src_c0 % 8) == 0 &&
+    const bool k64_ok = wk64 && p.cin == 64 && !p.upsample && !p.split && (p.src_cstride % 8) == 0 && (p.src_c0 % 8) == 0 &&
                         (p.mode == SRM_STORE_F16 || p.mode == SRM_ADD_STORE_F16 || p.mode == SRM_OUT_NCHW);
     if (sel == SRK_K64 || (sel == SRK_AUTO && sr_use_k64() && k64_ok)) {
         const int st = !k64_ok ? K4_ERR_UNSUPPORTED : (c.npad == 64) ? launch_conv_k64<64>(p, wk64, s)
@@ -1997,4 +2008,73 @@ extern "C" int k4_testing_sft(const k4_sft_test_args* a, int32_t* kernel_used, k
     k4_srnet_destroy(n);
     if (st == K4_OK && kernel_used) *kernel_used = used;
     return st;
+}
+
+// ------------------------------------------------------------------------------------------------
+// The decoder's 3x3 convolutions for another network: LPIPS's VGG16 trunk (k4_lpips.cu), in fp32-class precision from
+// fp16 operands.  A value x is carried as hi = fp16(x) and lo = fp16(x - hi) (both for activations and weights), and a
+// layer is the one GEMM of K = 3 Cin over the activation channels [hi | lo | hi] and the weights [w_hi | w_hi | w_lo]:
+// a_hi w_hi + a_lo w_hi + a_hi w_lo, only a_lo w_lo (2^-22 relative) dropped.  Cout is cut into blocks of 64 output
+// channels, each packed as the decoder packs a 64-channel conv and run by run_conv as one N = 64 launch whose epilogue
+// writes its channels of the three copies.
+// ------------------------------------------------------------------------------------------------
+namespace {
+// w [cout][cin][3][3] -> [cout][3 cin][3][3]: w_hi, w_hi, w_lo as fp32 values (each exact in fp16)
+__global__ void split_conv_weights_kernel(const float* __restrict__ w, float* __restrict__ dst, int cout, int cin) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)cout * 3 * cin * 9) return;
+    const int t = (int)(i % 9);
+    const long long r = i / 9;
+    const int k = (int)(r % (3 * cin)), co = (int)(r / (3 * cin));
+    const float v = w[((long long)co * cin + k % cin) * 9 + t];
+    const float hi = __half2float(__float2half_rn(v));
+    dst[i] = k < 2 * cin ? hi : __half2float(__float2half_rn(v - hi));
+}
+}  // namespace
+
+int k4_conv3x3_pack(const float* w, const float* b, int cout, int cin, cudaStream_t s, K4Conv3x3Pack* c) {
+    if (!w || !b || !c || cout < 64 || cout % 64 || cin < 1) return K4_ERR_INVALID_ARG;
+    *c = K4Conv3x3Pack{};
+    c->cout = cout;
+    c->cin = cin;
+    c->cin_pad = (3 * cin + 31) / 32 * 32;
+    const int nsl = c->cin_pad / SR_CK, nblk = cout / 64;
+    c->ws_bytes = (size_t)nsl * 9 * 64 * SR_CK * 2;                 // a multiple of 1024 B: every block stays aligned
+    const size_t nsplit = (size_t)cout * 3 * cin * 9;
+    K4_CUDA_TRY(cudaMalloc(&c->blob, nblk * c->ws_bytes + (size_t)cout * 4 + nsplit * 4));
+    unsigned char* blob = static_cast<unsigned char*>(c->blob);
+    c->wpack = blob;
+    c->bias = reinterpret_cast<float*>(blob + nblk * c->ws_bytes);
+    float* wsplit = c->bias + cout;                                  // staging of the split weights
+    split_conv_weights_kernel<<<(unsigned)((nsplit + 255) / 256), 256, 0, s>>>(w, wsplit, cout, cin);
+    for (int nb = 0; nb < nblk; ++nb) {
+        const long long total = (long long)nsl * 9 * 64 * SR_CK;
+        pack_conv3x3_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(wsplit + (size_t)nb * 64 * 3 * cin * 9,
+                                                                          c->wpack + nb * c->ws_bytes, 64, 3 * cin, 64, nsl);
+    }
+    K4_CUDA_TRY(cudaGetLastError());
+    K4_CUDA_TRY(cudaMemcpyAsync(c->bias, b, (size_t)cout * 4, cudaMemcpyDeviceToDevice, s));
+    return K4_OK;
+}
+
+void k4_conv3x3_free(K4Conv3x3Pack* c) {
+    if (c && c->blob) cudaFree(c->blob);
+    if (c) *c = K4Conv3x3Pack{};
+}
+
+int k4_conv3x3_relu_split(const K4Conv3x3Pack& c, const __half* src, int H, int W, __half* dst, cudaStream_t s) {
+    for (int nb = 0; nb < c.cout / 64; ++nb) {
+        SrConv sc{};
+        sc.wpack = c.wpack + nb * c.ws_bytes;
+        sc.bias = c.bias + 64 * nb;
+        sc.cin_pad = c.cin_pad;
+        sc.cout = sc.npad = 64;
+        ConvParams p{};
+        p.src = src; p.src_cstride = c.cin_pad; p.src_c0 = 0;
+        p.H = H; p.W = W;
+        p.mode = SRM_STORE_F16; p.relu = 1; p.split = c.cout;
+        p.dst_h = dst; p.dst_cstride = 3 * c.cout; p.dst_c0 = 64 * nb;
+        if (int st = run_conv(sc, p, s)) return st;
+    }
+    return K4_OK;
 }

@@ -2,14 +2,14 @@
 
 Differences that do not change results: rays are generated on the device (k4_make_rays), the whole
 frame is ONE fused launch instead of 8192-ray chunks (the chunk loop only bounds the reference's
-intermediate memory, run_sr.py:121-124), SSIM is computed on the device (utils.rgb_ssim of CUDA tensors), and
-LPIPS, which needs pretrained weights this project does not ship, raises if requested.
+intermediate memory, run_sr.py:121-124), and SSIM and LPIPS are computed on the device (utils.rgb_ssim and
+utils.rgb_lpips of CUDA tensors).
 """
 import numpy as np
 import torch
 
 from . import dvgo
-from .utils import rgb_ssim, to8b
+from .utils import rgb_lpips, rgb_ssim, to8b
 
 
 @torch.no_grad()
@@ -67,18 +67,29 @@ def _write_png(filename, rgb8):
     cv2.imwrite(filename, rgb8[..., ::-1])
 
 
-def _ssim_on_device(rgb, gt):
-    """``rgb_ssim(rgb, gt, max_val=1)`` of a clamped frame still on the device (run.py:134-135): the ground truth is
-    uploaded, the frame is not copied back for it."""
-    return rgb_ssim(rgb, torch.as_tensor(gt, device=rgb.device), max_val=1)
+def _score(rgb, gt, eval_ssim, eval_lpips_alex, eval_lpips_vgg, ssims, lpips_alex, lpips_vgg):
+    """run.py:136-141 / run_sr.py:146-151 on a clamped frame still on the device: the ground truth is uploaded once."""
+    if not (eval_ssim or eval_lpips_alex or eval_lpips_vgg):
+        return
+    gt = torch.as_tensor(gt, device=rgb.device)
+    if eval_ssim:
+        ssims.append(rgb_ssim(rgb, gt, max_val=1))
+    if eval_lpips_alex:
+        lpips_alex.append(rgb_lpips(rgb, gt, net_name='alex', device=rgb.device))
+    if eval_lpips_vgg:
+        lpips_vgg.append(rgb_lpips(rgb, gt, net_name='vgg', device=rgb.device))
 
 
-def _report(psnrs, ssims):
-    """run.py:141-145 / run_sr.py:153-157."""
+def _report(psnrs, ssims, lpips_vgg, lpips_alex):
+    """run.py:143-147 / run_sr.py:153-157."""
     if len(psnrs):
         print('Testing psnr', np.mean(psnrs), '(avg)')
         if len(ssims):
             print('Testing ssim', np.mean(ssims), '(avg)')
+        if len(lpips_vgg):
+            print('Testing lpips (vgg)', np.mean(lpips_vgg), '(avg)')
+        if len(lpips_alex):
+            print('Testing lpips (alex)', np.mean(lpips_alex), '(avg)')
 
 
 def _dump(rgbs, savedir, dump_images, global_step):
@@ -101,17 +112,15 @@ def render_viewpoints(model, render_poses, HW, Ks, ndc, render_kwargs,
 
     The reference reads ``cfg.data.flip_x/flip_y`` from a module global (run.py:96); here they come
     from ``render_kwargs`` unless passed explicitly.  The reference's defaults evaluate SSIM and LPIPS-VGG when ground
-    truth is given (here both default to off): ``eval_ssim`` scores the frame on the GPU (``utils.rgb_ssim``), LPIPS needs the
-    ``lpips`` package and its pretrained VGG / AlexNet weights and raises."""
+    truth is given (here both default to off): ``eval_ssim`` and ``eval_lpips_vgg`` / ``eval_lpips_alex`` score the
+    frame on the GPU (``utils.rgb_ssim``, ``utils.rgb_lpips``; LPIPS loads the ``lpips`` package's pretrained weights)."""
     assert len(render_poses) == len(HW) and len(HW) == len(Ks)
-    if eval_lpips_alex or eval_lpips_vgg:
-        raise NotImplementedError('LPIPS evaluation needs the lpips package and its pretrained weights')
     if arr_index is not None or img_enc is not None:
         raise NotImplementedError('img_enc conditioning needs lib/img_encoder, which the reference does not ship')
     flip_x = render_kwargs.get('flip_x', False) if flip_x is None else flip_x
     flip_y = render_kwargs.get('flip_y', False) if flip_y is None else flip_y
     frames = _render_frames(model, render_poses, HW, Ks, ndc, render_kwargs, render_factor, flip_x, flip_y)
-    rgbs, depths, bgmaps, psnrs, ssims = [], [], [], [], []
+    rgbs, depths, bgmaps, psnrs, ssims, lpips_alex, lpips_vgg = [], [], [], [], [], [], []
     for i, f in enumerate(frames):
         rgb_d = f['rgb_marched'].clamp(0, 1)
         rgb = rgb_d.cpu().numpy()
@@ -120,12 +129,11 @@ def render_viewpoints(model, render_poses, HW, Ks, ndc, render_kwargs,
         bgmaps.append(f['alphainv_last'].cpu().numpy())
         if gt_imgs is not None and render_factor == 0:
             psnrs.append(-10. * np.log10(np.mean(np.square(rgb - gt_imgs[i]))))
-            if eval_ssim:
-                ssims.append(_ssim_on_device(rgb_d, gt_imgs[i]))          # run.py:134-135
-    _report(psnrs, ssims)
+            _score(rgb_d, gt_imgs[i], eval_ssim, eval_lpips_alex, eval_lpips_vgg, ssims, lpips_alex, lpips_vgg)
+    _report(psnrs, ssims, lpips_vgg, lpips_alex)
     _post(rgbs, depths, bgmaps, render_video_flipy, render_video_rot90)
     _dump(rgbs, savedir, dump_images, global_step)
-    return np.array(rgbs), np.array(depths), np.array(bgmaps), psnrs, ssims, []
+    return np.array(rgbs), np.array(depths), np.array(bgmaps), psnrs, ssims, lpips_vgg
 
 
 @torch.no_grad()
@@ -142,9 +150,8 @@ def render_viewpoints_sr(model, render_poses, HW, Ks, ndc, render_kwargs,
     flip_x = render_kwargs.get('flip_x', False) if flip_x is None else flip_x
     flip_y = render_kwargs.get('flip_y', False) if flip_y is None else flip_y
     frames = _render_frames(model, render_poses, HW, Ks, ndc, render_kwargs, render_factor, flip_x, flip_y)
-    if eval_lpips_alex or eval_lpips_vgg:
-        raise NotImplementedError('LPIPS evaluation needs the lpips package and its pretrained weights')
     rgbs, rgb_features, depths, bgmaps, psnrs, ssims, viewdirs_all = [], [], [], [], [], [], []
+    lpips_alex, lpips_vgg = [], []
     for i, f in enumerate(frames):
         rgb_d = f['rgb_marched'].clamp(0, 1)
         rgb = rgb_d.cpu().numpy()
@@ -155,9 +162,9 @@ def render_viewpoints_sr(model, render_poses, HW, Ks, ndc, render_kwargs,
         viewdirs_all.append(f['viewdirs'])
         if gt_imgs is not None and render_factor == 0:
             psnrs.append(-10. * np.log10(np.mean(np.square(rgb - gt_imgs[i]))))
-            if eval_ssim:
-                ssims.append(_ssim_on_device(rgb_d, gt_imgs[i]))          # run_sr.py:146-147 (printed, not returned)
-    _report(psnrs, ssims)
+            # run_sr.py:146-151: printed, not returned
+            _score(rgb_d, gt_imgs[i], eval_ssim, eval_lpips_alex, eval_lpips_vgg, ssims, lpips_alex, lpips_vgg)
+    _report(psnrs, ssims, lpips_vgg, lpips_alex)
     _post(rgbs, depths, bgmaps, render_video_flipy, render_video_rot90)
     _dump(rgbs, savedir, dump_images, global_step)
     return np.array(rgbs), np.array(depths), np.array(bgmaps), psnrs, viewdirs_all, np.array(rgb_features)

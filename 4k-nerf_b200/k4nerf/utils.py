@@ -100,6 +100,113 @@ def rgb_ssim(img0, img1, max_val, filter_size=11, filter_sigma=1.5, k1=0.01, k2=
 
 
 # ------------------------------------------------------------------------------------------------
+# LPIPS (lib/utils.py:137-149)
+# ------------------------------------------------------------------------------------------------
+_LPIPS_NETS = {'vgg': 0, 'alex': 1}                                 # K4_LPIPS_VGG / K4_LPIPS_ALEX
+_LPIPS_CONVS = {
+    'vgg': ['net.slice1.0', 'net.slice1.2', 'net.slice2.5', 'net.slice2.7', 'net.slice3.10', 'net.slice3.12',
+            'net.slice3.14', 'net.slice4.17', 'net.slice4.19', 'net.slice4.21', 'net.slice5.24', 'net.slice5.26',
+            'net.slice5.28'],
+    'alex': ['net.slice1.0', 'net.slice2.3', 'net.slice3.6', 'net.slice4.8', 'net.slice5.10'],
+}
+_LPIPS_SHIFT, _LPIPS_SCALE = (-.030, -.088, -.188), (.458, .448, .450)
+__LPIPS__ = {}
+
+
+def _lpips_state_dict(net_name):
+    """The pretrained weights, as the reference's init_lpips builds its module (needs the ``lpips`` package)."""
+    import lpips
+    print(f'init_lpips: lpips_{net_name}')
+    return lpips.LPIPS(net=net_name, version='0.1').state_dict()
+
+
+class LpipsNet:
+    """``lpips.LPIPS(net=net_name, version='0.1')`` on one CUDA device (``k4_lpips_create``, csrc/k4_lpips.cu) from a
+    state dict with its keys (``net.slice*``, ``lin0..4.model.1.weight``; a ``scaling_layer`` must hold lpips' own
+    constants)."""
+
+    def __init__(self, net_name, state_dict, device):
+        import ctypes as C
+        from . import _lib
+        if net_name not in _LPIPS_NETS:
+            raise ValueError(f"rgb_lpips: net_name must be 'vgg' or 'alex', got {net_name!r}")
+        for k, ref in (('scaling_layer.shift', _LPIPS_SHIFT), ('scaling_layer.scale', _LPIPS_SCALE)):
+            if k in state_dict and not torch.equal(state_dict[k].detach().float().cpu().view(-1), torch.tensor(ref)):
+                raise ValueError(f'rgb_lpips: {k} differs from lpips 0.1\'s constants {ref}')
+        keys = [k + s for k in _LPIPS_CONVS[net_name] for s in ('.weight', '.bias')] + [f'lin{i}.model.1.weight' for i in range(5)]
+        missing = [k for k in keys if k not in state_dict]
+        if missing:
+            raise KeyError(f'rgb_lpips: the state dict lacks {missing}')
+        self.net_name, self.device, self._lib, self.handle = net_name, device, _lib, None
+        params = [state_dict[k].detach().to(device=device, dtype=torch.float32).contiguous() for k in keys]
+        ptrs = (C.c_void_p * len(params))(*[p.data_ptr() for p in params])
+        h = C.c_void_p()
+        with torch.cuda.device(device):
+            _lib.check(_lib.lib.k4_lpips_create(_LPIPS_NETS[net_name], ptrs, len(params),
+                                                C.c_void_p(torch.cuda.current_stream(device).cuda_stream), C.byref(h)),
+                       'k4_lpips_create')
+        self.handle = h
+
+    def __del__(self):
+        if getattr(self, 'handle', None) is not None:
+            self._lib.lib.k4_lpips_destroy(self.handle)
+            self.handle = None
+
+    def __call__(self, img0, img1):
+        """The score of two ``[H, W, 3]`` float32 CUDA images on this device (any strides) as a Python float."""
+        import ctypes as C
+        H, W = img0.shape[0], img0.shape[1]
+        with torch.cuda.device(self.device):
+            ws = torch.empty(self._lib.lib.k4_lpips_workspace_bytes(self.handle, H, W), dtype=torch.uint8, device=self.device)
+            if ws.numel() == 0:
+                raise ValueError(f'rgb_lpips: {H} x {W} is outside what lpips {self.net_name} takes '
+                                 f'({"16" if self.net_name == "vgg" else "31"} .. 16384 pixels per side)')
+            out = torch.empty((), dtype=torch.float64, device=self.device)
+            self._lib.check(self._lib.lib.k4_lpips_forward(
+                self.handle, C.c_void_p(img0.data_ptr()), C.c_void_p(img1.data_ptr()), _strides3(img0), _strides3(img1),
+                H, W, C.c_void_p(out.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(),
+                C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)), 'k4_lpips_forward')
+        return float(out.item())
+
+
+def rgb_lpips(np_gt, np_im, net_name, device=None, weights=None):
+    """LPIPS 0.1 of two ``[H, W, 3]`` images in [0, 1] as ``lib/utils.py:144-149`` computes it
+    (``lpips.LPIPS(net=net_name, version='0.1')(gt, im, normalize=True).item()``), on the GPU (csrc/k4_lpips.cu):
+    VGG16's convolutions on the decoder's wgmma kernels with every value an fp16 pair hi + lo (fp32-class), AlexNet's
+    in fp32, the head in fp64.  The score is a float, bitwise reproducible.
+
+    ``np_gt``, ``np_im``: numpy arrays, or tensors of any strides (e.g. ``sr.permute(1, 2, 0)`` of a ``[3, H, W]`` 4K
+    frame, scored in place when it is float32 on the GPU).  ``device``: where to score; CUDA tensors are scored on
+    their own device.  ``weights``: a state dict with ``lpips.LPIPS``' keys; by default the pretrained weights of the
+    ``lpips`` package, loaded once per net and device (without the package this raises ``ImportError``, as the
+    reference does)."""
+    cuda_in = [t for t in (np_gt, np_im) if _is_cuda(t)]
+    dev = cuda_in[0].device if cuda_in else torch.device(device if device is not None else 'cuda')
+    if dev.type != 'cuda':
+        raise ValueError(f'rgb_lpips runs on a CUDA device (got {dev})')
+    if dev.index is None:
+        dev = torch.device('cuda', torch.cuda.current_device())
+    if weights is None:
+        key = (net_name, dev)
+        if key not in __LPIPS__:
+            __LPIPS__[key] = LpipsNet(net_name, _lpips_state_dict(net_name), dev)
+        net = __LPIPS__[key]
+    else:
+        net = LpipsNet(net_name, weights, dev)
+
+    def as_image(x):
+        x = torch.from_numpy(np.asarray(x)) if not isinstance(x, torch.Tensor) else x.detach()
+        if x.ndim != 3 or x.shape[-1] != 3:
+            raise ValueError(f'rgb_lpips: [H, W, 3] images expected, got shape {tuple(x.shape)}')
+        return x.to(device=dev, dtype=torch.float32)
+
+    img0, img1 = as_image(np_gt), as_image(np_im)
+    if img0.shape != img1.shape:
+        raise ValueError(f'rgb_lpips: the images differ in shape: {tuple(img0.shape)} and {tuple(img1.shape)}')
+    return net(img0, img1)
+
+
+# ------------------------------------------------------------------------------------------------
 # The depth video of run_sr.py --render_video (run_sr.py:1459-1463)
 # ------------------------------------------------------------------------------------------------
 def rainbow_lut_u8():

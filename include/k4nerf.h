@@ -493,6 +493,46 @@ K4_API int k4_op_rgb_ssim(const void* d_img0, const void* d_img1, int32_t dtype,
                           double* d_map, double* d_mean, void* d_workspace, size_t workspace_bytes, k4_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * LPIPS (csrc/k4_lpips.cu).
+ *
+ * Replaces: utils.rgb_lpips (lib/utils.py:137-149), lpips.LPIPS(net='vgg' | 'alex', version='0.1') called with
+ * normalize=True, the perceptual metric of render_viewpoints' eval_lpips_vgg / eval_lpips_alex.
+ *
+ * k4_lpips_create: h_params is a HOST array of n_params DEVICE pointers to fp32 parameters, in this fixed order (the
+ * keys of lpips.LPIPS(...).state_dict()):
+ *   K4_LPIPS_VGG  (n_params 31): net.slice1.{0,2}, net.slice2.{5,7}, net.slice3.{10,12,14}, net.slice4.{17,19,21},
+ *                 net.slice5.{24,26,28}, each .weight [cout][cin][3][3] then .bias [cout]; then lin0 .. lin4
+ *                 .model.1.weight ([1][C][1][1], C = 64, 128, 256, 512, 512).
+ *   K4_LPIPS_ALEX (n_params 15): net.slice1.0, net.slice2.3, net.slice3.6, net.slice4.8, net.slice5.10, each .weight
+ *                 then .bias; then lin0 .. lin4 .model.1.weight (C = 64, 192, 384, 256, 256).
+ * The scaling layer's shift (-.030, -.088, -.188) and scale (.458, .448, .450) are lpips' constants, built in.  The
+ * parameters are copied (the call synchronises `stream`, so they may be freed on return).  A NULL pointer, another
+ * net or another n_params: K4_ERR_INVALID_ARG, before any CUDA call.
+ *
+ * k4_lpips_forward: d_img0, d_img1: two H x W x 3 fp32 images in [0, 1], element (y, x, c) at y * strides[0] +
+ * x * strides[1] + c * strides[2] (HOST arrays of element strides, so [H, W, 3] and [3, H, W] tensors and views are read
+ * in place).  *d_out (one device double) receives the score: the sum over the five taps of the mean over the tap's
+ * pixels of sum_c lin[c] (f0 / (|f0| + 1e-10) - f1 / (|f1| + 1e-10))^2, |f| the L2 norm of a pixel's channel vector.
+ * VGG's convolutions run on the tensor cores with every activation and weight an fp16 pair hi + lo (three fp16 GEMM
+ * terms, fp32 accumulation: fp32-class), AlexNet's in fp32; the head is fp64, summed in an order fixed by (net, H, W),
+ * so the score is bitwise reproducible.  Caller's stream, no host sync.  The workspace holds
+ * k4_lpips_workspace_bytes(net, H, W) bytes (0 for a size the trunk cannot take: VGG needs H, W >= 16, AlexNet
+ * H, W >= 31; both at most 16384), 256-byte aligned.  A NULL pointer, a size outside those bounds or a misaligned
+ * pointer: K4_ERR_INVALID_ARG; a workspace smaller than the size: K4_ERR_WORKSPACE; both before any CUDA call.
+ */
+enum { K4_LPIPS_VGG = 0, K4_LPIPS_ALEX = 1 };
+typedef struct k4_lpips k4_lpips;
+/* Replaces: lpips.LPIPS(net=..., version='0.1') (lib/utils.py:138-142). */
+K4_API int k4_lpips_create(int32_t net, const float* const* h_params, int32_t n_params, k4_stream_t stream, k4_lpips** out_net);
+K4_API int k4_lpips_destroy(k4_lpips* net);
+/* Replaces: utils.rgb_lpips (lib/utils.py:144-149) -- the workspace of k4_lpips_forward. */
+K4_API size_t k4_lpips_workspace_bytes(const k4_lpips* net, int64_t H, int64_t W);
+/* Replaces: utils.rgb_lpips (lib/utils.py:144-149). */
+K4_API int k4_lpips_forward(const k4_lpips* net, const float* d_img0, const float* d_img1, const int64_t strides0[3],
+                            const int64_t strides1[3], int64_t H, int64_t W, double* d_out, void* d_workspace,
+                            size_t workspace_bytes, k4_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Video streams of run_sr.py --render_video (csrc/k4_video.cu).
  *
  * k4_op_masked_quantiles replaces the depth video's range, run_sr.py:1459-1461:
@@ -800,6 +840,21 @@ K4_API int k4_testing_march_phases(const k4_scene* scene, const k4_render_args* 
  *   is a synchronous cudaMemcpy: the call returns when d_out holds the field.
  */
 K4_API int k4_testing_skip_field(const k4_scene* scene, uint8_t* d_out, int64_t n, int32_t cdims[3]);
+
+/*
+ * k4_testing_lpips_stage: one image through k4_lpips_forward's trunk up to `stage`, so that a test can compare each
+ * layer with a reference.  Stage 0 is the scaled input (2x - 1, then the scaling layer); stage s >= 1 is the output of
+ * the trunk's s-th operation, in the order of torchvision's features: VGG16 17 (conv + ReLU, or 2x2 max-pool), AlexNet
+ * 7 (conv + ReLU, or 3x3 / 2 max-pool).  out_shape (host) receives the stored (h, w, c); d_out (NULL: only the shape)
+ * receives the stage as h x w x c contiguous: for VGG fp16 with c = 3 C, the pairs hi = fp16(x), lo = fp16(x - hi) of
+ * the C channels as [hi | lo | hi] (stage 0: 32 channels, hi, lo, hi of the image's 3, then zeros), for AlexNet fp32
+ * with c = C.
+ * Image, strides, size and workspace as k4_lpips_forward (one image's half of the workspace is used).  Arguments are
+ * checked before any CUDA call (K4_ERR_INVALID_ARG, K4_ERR_WORKSPACE).  Caller's stream, no host sync.
+ */
+K4_API int k4_testing_lpips_stage(const k4_lpips* net, const float* d_img, const int64_t strides[3], int64_t H, int64_t W,
+                                  int32_t stage, void* d_out, int64_t out_shape[3], void* d_workspace, size_t workspace_bytes,
+                                  k4_stream_t stream);
 
 #ifdef __cplusplus
 }
