@@ -15,6 +15,11 @@
 //     vq_hist_kernel<2>     the last 10 bits
 //     vq_select_kernel<2>   the four keys, then numpy's _lerp in fp64
 //   Counts are integers added by atomics, so the selected keys, and the results, are exact and bitwise reproducible.
+//   Because integer histograms add exactly, the passes also run split (k4_op_masked_quantiles_hist / _select): every
+//   rank adds its own frames into a caller-visible int64 histogram, the callers sum the histograms (an all-reduce), and
+//   every rank runs the same select on the sum, so all ranks carry the same state into the next pass.  The histogram is
+//   the fused op's [VQ_RANKS][VQ_BINS] plus, in pass 0, the count and the NaN count (the fused op keeps those two in its
+//   state instead).
 //
 // Depth-video frames: x = 1 - clip((depths_vis - dmin) / (dmax - dmin), 0, 1) in fp64, matplotlib's Colormap.__call__
 // index (trunc(256 x), 256 -> 255, NaN -> the 'bad' colour 0), then the host's u8 table (to8b of the colormap's rgb).
@@ -50,6 +55,7 @@ struct VqArgs {
     double q[2];
     VqState* st;
     unsigned long long* hist;                  // [VQ_RANKS][VQ_BINS]
+    unsigned long long* tally;                 // pass 0's count and NaN count: st->count / nans, or after hist's bins
     double* out;                               // [2]
     long long* count;
 };
@@ -128,8 +134,8 @@ __global__ void __launch_bounds__(VQ_NT) vq_hist_kernel(const __grid_constant__ 
         if (tid == 0) {
             unsigned long long c = 0, m = 0;
             for (int i = 0; i < VQ_NT / 32; ++i) { c += sred[0][i]; m += sred[1][i]; }
-            if (c) atomicAdd(&a.st->count, c);
-            if (m) atomicAdd(&a.st->nans, m);
+            if (c) atomicAdd(&a.tally[0], c);
+            if (m) atomicAdd(&a.tally[1], m);
         }
     }
 }
@@ -147,7 +153,7 @@ template <int P>
 __global__ void __launch_bounds__(32 * VQ_RANKS) vq_select_kernel(const __grid_constant__ VqArgs a) {
     VqState* st = a.st;
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const unsigned long long n = st->count;
+    const unsigned long long n = P == 0 ? a.tally[0] : st->count;
     if (P == 0 && threadIdx.x == 0) {
         for (int j = 0; j < 2; ++j) {
             unsigned long long prev = 0, next = 0;
@@ -202,6 +208,10 @@ __global__ void __launch_bounds__(32 * VQ_RANKS) vq_select_kernel(const __grid_c
     }
     __syncthreads();
     if (threadIdx.x == 0) {
+        if (P == 0) {                                           // the tally into the state (a no-op in the fused op)
+            st->count = n;
+            st->nans = a.tally[1];
+        }
         if (P < 2) {
             for (int r = 0; r < VQ_RANKS; ++r) {
                 int k = 0;
@@ -297,6 +307,7 @@ __global__ void __launch_bounds__(DV_NT) frame_u8_kernel(const __grid_constant__
 }
 
 constexpr long long VQ_MAX_ROWS = 0x7fffffffLL;
+static_assert(K4_MASKED_QUANTILES_HIST_LEN == VQ_RANKS * VQ_BINS + 2, "the header's histogram length");
 
 bool vq_shape_ok(int64_t n, int64_t H, int64_t W) {
     return n >= 1 && H >= 1 && W >= 1 && n <= VQ_MAX_ROWS && H <= VQ_MAX_ROWS && W <= VQ_MAX_ROWS && n * H <= VQ_MAX_ROWS;
@@ -306,6 +317,35 @@ bool vq_shape_ok(int64_t n, int64_t H, int64_t W) {
 bool frame_shape_ok(int64_t n, int64_t H, int64_t W) {
     return n >= 1 && H >= 1 && W >= 1 && n <= 65535 && H <= 65535 && W <= 65535;
 }
+
+VqArgs vq_args(const float* d_depth, const float* d_bgmap, int64_t n, int64_t H, int64_t W, const int64_t depth_strides[3],
+               const int64_t bgmap_strides[3], void* d_state) {
+    VqArgs a{};
+    a.depth = d_depth;
+    a.bg = d_bgmap;
+    for (int i = 0; i < 3; ++i) { a.sd[i] = depth_strides[i]; a.sb[i] = bgmap_strides[i]; }
+    a.n = n;
+    a.H = H;
+    a.W = W;
+    a.rows = n * H;
+    a.st = (VqState*)d_state;
+    return a;
+}
+
+void vq_hist(int pass, const VqArgs& a, cudaStream_t s) {
+    const unsigned grid = (unsigned)std::min<long long>(a.rows, VQ_MAX_CTAS);
+    if (pass == 0) vq_hist_kernel<0><<<grid, VQ_NT, 0, s>>>(a);
+    else if (pass == 1) vq_hist_kernel<1><<<grid, VQ_NT, 0, s>>>(a);
+    else vq_hist_kernel<2><<<grid, VQ_NT, 0, s>>>(a);
+}
+
+void vq_select(int pass, const VqArgs& a, cudaStream_t s) {
+    if (pass == 0) vq_select_kernel<0><<<1, 32 * VQ_RANKS, 0, s>>>(a);
+    else if (pass == 1) vq_select_kernel<1><<<1, 32 * VQ_RANKS, 0, s>>>(a);
+    else vq_select_kernel<2><<<1, 32 * VQ_RANKS, 0, s>>>(a);
+}
+
+bool q_ok(const double q[2]) { return q[0] >= 0.0 && q[0] <= 1.0 && q[1] >= 0.0 && q[1] <= 1.0; }
 
 int rot_k(int32_t rot90) { return ((rot90 % 4) + 4) % 4; }
 
@@ -330,41 +370,67 @@ int k4_op_masked_quantiles(const float* d_depth, const float* d_bgmap, int64_t n
                            k4_stream_t stream) {
     if (!d_depth || !d_bgmap || !depth_strides || !bgmap_strides || !h_q || !d_quantiles || !d_count || !d_workspace)
         return K4_ERR_INVALID_ARG;
-    if (!vq_shape_ok(n, H, W)) return K4_ERR_INVALID_ARG;
-    for (int j = 0; j < 2; ++j)
-        if (!(h_q[j] >= 0.0 && h_q[j] <= 1.0)) return K4_ERR_INVALID_ARG;
+    if (!vq_shape_ok(n, H, W) || !q_ok(h_q)) return K4_ERR_INVALID_ARG;
     if ((uintptr_t)d_workspace % 16 || (uintptr_t)d_quantiles % sizeof(double) || (uintptr_t)d_count % sizeof(int64_t) ||
         (uintptr_t)d_depth % sizeof(float) || (uintptr_t)d_bgmap % sizeof(float))
         return K4_ERR_INVALID_ARG;
     if (workspace_bytes < k4_op_masked_quantiles_workspace_bytes(n, H, W)) return K4_ERR_WORKSPACE;
-    VqArgs a{};
-    a.depth = d_depth;
-    a.bg = d_bgmap;
-    for (int i = 0; i < 3; ++i) { a.sd[i] = depth_strides[i]; a.sb[i] = bgmap_strides[i]; }
-    a.n = n;
-    a.H = H;
-    a.W = W;
-    a.rows = n * H;
+    VqArgs a = vq_args(d_depth, d_bgmap, n, H, W, depth_strides, bgmap_strides, d_workspace);
     a.q[0] = h_q[0];
     a.q[1] = h_q[1];
-    a.st = (VqState*)d_workspace;
     a.hist = (unsigned long long*)((char*)d_workspace + VQ_STATE_BYTES);
+    a.tally = &a.st->count;
     a.out = d_quantiles;
     a.count = (long long*)d_count;
     cudaStream_t s = (cudaStream_t)stream;
-    const unsigned grid = (unsigned)std::min<long long>(a.rows, VQ_MAX_CTAS);
     const size_t hist_bytes = sizeof(unsigned long long) * VQ_RANKS * VQ_BINS;
     // pass 0 fills histogram 0; before passes 1 and 2 the select kernel has read it, so the next pass starts from zero
     K4_CUDA_TRY(cudaMemsetAsync(d_workspace, 0, VQ_STATE_BYTES + hist_bytes, s));
-    vq_hist_kernel<0><<<grid, VQ_NT, 0, s>>>(a);
-    vq_select_kernel<0><<<1, 32 * VQ_RANKS, 0, s>>>(a);
-    K4_CUDA_TRY(cudaMemsetAsync(a.hist, 0, hist_bytes, s));
-    vq_hist_kernel<1><<<grid, VQ_NT, 0, s>>>(a);
-    vq_select_kernel<1><<<1, 32 * VQ_RANKS, 0, s>>>(a);
-    K4_CUDA_TRY(cudaMemsetAsync(a.hist, 0, hist_bytes, s));
-    vq_hist_kernel<2><<<grid, VQ_NT, 0, s>>>(a);
-    vq_select_kernel<2><<<1, 32 * VQ_RANKS, 0, s>>>(a);
+    for (int p = 0; p < 3; ++p) {
+        if (p) K4_CUDA_TRY(cudaMemsetAsync(a.hist, 0, hist_bytes, s));
+        vq_hist(p, a, s);
+        vq_select(p, a, s);
+    }
     return launch_error("k4_op_masked_quantiles launch");
+}
+
+size_t k4_op_masked_quantiles_pass_workspace_bytes(void) { return VQ_STATE_BYTES; }
+
+int k4_op_masked_quantiles_hist(int32_t pass, const float* d_depth, const float* d_bgmap, int64_t n, int64_t H, int64_t W,
+                                const int64_t depth_strides[3], const int64_t bgmap_strides[3], int64_t* d_hist,
+                                const void* d_workspace, size_t workspace_bytes, k4_stream_t stream) {
+    if (pass < 0 || pass > 2 || !depth_strides || !bgmap_strides || !d_hist || !d_workspace) return K4_ERR_INVALID_ARG;
+    if (n < 0 || !vq_shape_ok(n ? n : 1, H, W)) return K4_ERR_INVALID_ARG;       // a share may hold no frames
+    if (n && (!d_depth || !d_bgmap || (uintptr_t)d_depth % sizeof(float) || (uintptr_t)d_bgmap % sizeof(float)))
+        return K4_ERR_INVALID_ARG;
+    if ((uintptr_t)d_workspace % 16 || (uintptr_t)d_hist % sizeof(int64_t)) return K4_ERR_INVALID_ARG;
+    if (workspace_bytes < VQ_STATE_BYTES) return K4_ERR_WORKSPACE;
+    if (n == 0) return K4_OK;
+    VqArgs a = vq_args(d_depth, d_bgmap, n, H, W, depth_strides, bgmap_strides, const_cast<void*>(d_workspace));
+    a.hist = (unsigned long long*)d_hist;
+    a.tally = a.hist + VQ_RANKS * VQ_BINS;
+    vq_hist(pass, a, (cudaStream_t)stream);
+    return launch_error("k4_op_masked_quantiles_hist launch");
+}
+
+int k4_op_masked_quantiles_select(int32_t pass, const int64_t* d_hist, const double h_q[2], double* d_quantiles,
+                                  int64_t* d_count, void* d_workspace, size_t workspace_bytes, k4_stream_t stream) {
+    if (pass < 0 || pass > 2 || !d_hist || !h_q || !d_quantiles || !d_count || !d_workspace) return K4_ERR_INVALID_ARG;
+    if (!q_ok(h_q)) return K4_ERR_INVALID_ARG;
+    if ((uintptr_t)d_workspace % 16 || (uintptr_t)d_hist % sizeof(int64_t) || (uintptr_t)d_quantiles % sizeof(double) ||
+        (uintptr_t)d_count % sizeof(int64_t))
+        return K4_ERR_INVALID_ARG;
+    if (workspace_bytes < VQ_STATE_BYTES) return K4_ERR_WORKSPACE;
+    VqArgs a{};
+    a.q[0] = h_q[0];
+    a.q[1] = h_q[1];
+    a.st = (VqState*)d_workspace;
+    a.hist = (unsigned long long*)const_cast<int64_t*>(d_hist);          // read only: the select reads the histogram
+    a.tally = a.hist + VQ_RANKS * VQ_BINS;
+    a.out = d_quantiles;
+    a.count = (long long*)d_count;
+    vq_select(pass, a, (cudaStream_t)stream);
+    return launch_error("k4_op_masked_quantiles_select launch");
 }
 
 int k4_op_depth_video_u8(const float* d_depth, const float* d_bgmap, int64_t n, int64_t H, int64_t W,

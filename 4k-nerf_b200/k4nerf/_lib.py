@@ -11,6 +11,7 @@ K4_MLP_FP32, K4_MLP_F16, K4_MLP_F16X3, K4_MLP_TCGEN05, K4_MLP_TCGEN05_WS = 0, 1,
 K4_ACT_RELU, K4_ACT_GAUSS, K4_ACT_LKRELU = 0, 1, 2
 K4_MAX_MLP_LAYERS = 8
 K4_MAX_PEERS = 8
+K4_MASKED_QUANTILES_HIST_LEN = 4 * 2048 + 2
 MLP_MODES = {'fp32': K4_MLP_FP32, 'f16': K4_MLP_F16, 'f16x3': K4_MLP_F16X3, 'tcgen05': K4_MLP_TCGEN05,
              'tc': K4_MLP_TCGEN05, 'ws': K4_MLP_TCGEN05_WS}
 
@@ -231,6 +232,12 @@ EXPORTS = {
     'k4_op_masked_quantiles': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.POINTER(C.c_int64),
                                          C.POINTER(C.c_int64), C.POINTER(C.c_double), C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_size_t, C.c_void_p]),
+    'k4_op_masked_quantiles_pass_workspace_bytes': (C.c_size_t, []),
+    'k4_op_masked_quantiles_hist': (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
+                                              C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_void_p, C.c_void_p,
+                                              C.c_size_t, C.c_void_p]),
+    'k4_op_masked_quantiles_select': (C.c_int, [C.c_int32, C.c_void_p, C.POINTER(C.c_double), C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_size_t, C.c_void_p]),
     'k4_op_depth_video_u8': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.POINTER(C.c_int64),
                                        C.POINTER(C.c_int64), C.c_void_p, C.POINTER(C.c_uint8), C.c_int32, C.c_int32,
                                        C.c_void_p, C.c_void_p]),

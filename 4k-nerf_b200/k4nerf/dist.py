@@ -514,3 +514,95 @@ def sr_decode_sharded(net_fn, img, cond, tile_size, tile_pad=10, scale=4, halo=8
             output[0, :, y0 * s:y1 * s, x0 * s:x1 * s] = g[r, off:off + n].view(C, (y1 - y0) * s, (x1 - x0) * s)
             off += n
     return output
+
+
+# ------------------------------------------------------------------------------------------------
+# Video sharding: whole frames dealt round-robin over the ranks (frames are independent, so nothing but the finished
+# u8 frames and the depth video's histograms crosses GPUs).
+# ------------------------------------------------------------------------------------------------
+def _world_rank(group):
+    if not dist.is_initialized():
+        return 1, 0
+    return dist.get_world_size(group), dist.get_rank(group)
+
+
+def _via_host(t, group):
+    """gloo takes CUDA tensors through the host (its collectives here are CPU ones)."""
+    return t.is_cuda and dist.get_backend(group) == 'gloo'
+
+
+def all_reduce_sum(t, group=None):
+    """In-place ``all_reduce(SUM)`` of ``t`` over ``group`` (nothing without a process group or on one rank)."""
+    if _world_rank(group)[0] == 1:
+        return t
+    if _via_host(t, group):
+        h = t.cpu()
+        dist.all_reduce(h, group=group)
+        return t.copy_(h)
+    dist.all_reduce(t, group=group)
+    return t
+
+
+def gather_to(t, dst, group=None):
+    """``dist.gather`` of equal-shaped ``t`` from every rank of ``group`` to group rank ``dst``: the list of the ranks'
+    tensors (on ``t``'s device) on ``dst``, ``None`` elsewhere."""
+    world, rank = _world_rank(group)
+    if world == 1:
+        return [t]
+    src = t.cpu() if _via_host(t, group) else t
+    got = [torch.empty_like(src) for _ in range(world)] if rank == dst else None
+    dist.gather(src, got, dst=dist.get_global_rank(group, dst) if group is not None else dst, group=group)
+    return None if got is None else [g.to(t.device) for g in got]
+
+
+def render_video_frames(render_into, n, H, W, sr_shape, lr_shape, device, render_video_flipy=False, render_video_rot90=0,
+                        on_frame=None, group=None, dst=0):
+    """The three videos of ``n`` frames rendered across the ranks of ``group``, returned on group rank ``dst`` as
+    :func:`k4nerf.render.render_video_4k` returns them: ``(sr [n, *sr_shape], lr [n, *lr_shape], depth [n, H', W', 3])``
+    uint8 numpy arrays (``sr`` ``None`` with ``on_frame``); every other rank returns ``(None, None, None)``.
+
+    Frame ``i`` is rendered by rank ``i % world``: ``render_into(i, sr_u8, lr_u8, depth, bgmap)`` fills the frame's
+    uint8 SR and LR frames and its ``[H, W]`` float32 depth and bgmap.  Frames go round by round, one per rank: the
+    round's u8 frames are gathered to ``dst`` (one ``gather`` of a packed ``[sr | lr]`` buffer per round), where
+    ``on_frame(i, sr_u8, lr_u8)`` sees them in increasing ``i`` or the SR frame is copied to the host.  Each rank keeps
+    the depths and bgmaps of its own frames only; the depth video is made by
+    :func:`k4nerf.utils.depth_video_frames_sharded` under the range of all frames and gathered to ``dst`` at the end.
+    Collective: every rank of ``group`` calls it with the same arguments."""
+    import numpy as np
+    from .utils import depth_video_frames_sharded
+    world, rank = _world_rank(group)
+    if not 0 <= dst < world:
+        raise ValueError(f'render_video_frames: dst {dst} is not a rank of a group of {world}')
+    on_dst = rank == dst
+    S, L = int(np.prod(sr_shape)), int(np.prod(lr_shape))
+    mine = range(rank, n, world)
+    depths = torch.empty((len(mine), H, W), dtype=torch.float32, device=device)
+    bgmaps = torch.empty((len(mine), H, W), dtype=torch.float32, device=device)
+    if on_dst:
+        lr_u8 = torch.empty((n, *lr_shape), dtype=torch.uint8, device=device)
+        sr_host = None if on_frame is not None else np.empty((n, *sr_shape), dtype=np.uint8)
+    for r in range(len(range(0, n, world))):
+        send = torch.empty(S + L, dtype=torch.uint8, device=device)    # a fresh frame: on_frame may keep its sr_u8
+        if r < len(mine):
+            render_into(mine[r], send[:S].view(sr_shape), send[S:].view(lr_shape), depths[r], bgmaps[r])
+        got = gather_to(send, dst, group)
+        if not on_dst:
+            continue
+        for q, buf in enumerate(got[:n - r * world]):
+            i = r * world + q
+            lr_u8[i].copy_(buf[S:].view(lr_shape))
+            if on_frame is not None:
+                on_frame(i, buf[:S].view(sr_shape), lr_u8[i])
+            else:
+                torch.from_numpy(sr_host[i]).copy_(buf[:S].view(sr_shape))
+    mine_u8 = torch.as_tensor(depth_video_frames_sharded(depths, bgmaps, q=(5, 95), render_video_flipy=render_video_flipy,
+                                                         render_video_rot90=render_video_rot90, group=group))
+    send = torch.zeros((len(range(0, n, world)), *mine_u8.shape[1:]), dtype=torch.uint8, device=mine_u8.device)
+    send[:len(mine)] = mine_u8
+    got = gather_to(send, dst, group)
+    if not on_dst:
+        return None, None, None
+    depth_u8 = torch.empty((n, *mine_u8.shape[1:]), dtype=torch.uint8, device=mine_u8.device)
+    for q, frames in enumerate(got):
+        depth_u8[q::world] = frames[:len(range(q, n, world))]
+    return sr_host, lr_u8.cpu().numpy(), depth_u8.cpu().numpy()

@@ -253,6 +253,45 @@ def render_video_4k(model, net_sr, render_poses, HW, Ks, ndc, render_kwargs, ren
 
 
 @torch.no_grad()
+def render_video_4k_sharded(model, net_sr, render_poses, HW, Ks, ndc, render_kwargs, render_factor=0,
+                            render_video_flipy=False, render_video_rot90=0, test_tile=510, flip_x=None, flip_y=None,
+                            on_frame=None, group=None, dst=0):
+    """:func:`render_video_4k` on every rank of ``group`` (one process per GPU of one node, scene and decoder
+    replicated, as for :func:`render_frame_4k_sharded`): frame ``i`` is :func:`render_frame_4k` on rank ``i % world``,
+    whole, so ranks exchange no part of a frame (:func:`k4nerf.dist.render_video_frames`).  Rank ``dst`` returns
+    ``(sr, lr, depth)``, bit for bit :func:`render_video_4k`'s on the same inputs, and calls ``on_frame(i, sr_u8, lr_u8)``
+    in increasing ``i``; every other rank returns ``(None, None, None)``.  The u8 frames of each round (one frame per
+    rank) are gathered to ``dst``; the depth video's 5th / 95th percentiles are exact over all frames
+    (:func:`k4nerf.utils.depth_video_frames_sharded`: three histogram all-reduces).  A ``gloo`` group takes the CUDA
+    tensors through the host.  Collective: every rank calls it with the same arguments."""
+    from . import dist as kdist
+    from .utils import frame_u8_cuda
+    assert len(render_poses) == len(HW) and len(HW) == len(Ks)
+    flip_x = render_kwargs.get('flip_x', False) if flip_x is None else flip_x
+    flip_y = render_kwargs.get('flip_y', False) if flip_y is None else flip_y
+    if render_factor != 0:
+        HW = (np.copy(HW) / render_factor).astype(int)
+        Ks = np.copy(Ks)
+        Ks[:, :2, :3] /= render_factor
+    H, W = int(HW[0][0]), int(HW[0][1])
+    if any((int(h), int(w)) != (H, W) for h, w in HW):
+        raise ValueError('render_video_4k_sharded: every frame of a video must have the same size')
+    k = int(render_video_rot90) % 4
+    rot = lambda h, w: (w, h) if k & 1 else (h, w)
+    s = net_sr.scale
+
+    def render_into(i, sr_u8, lr_u8, depth, bgmap):
+        sr, lr = render_frame_4k(model, net_sr, H, W, Ks[i], render_poses[i], ndc, render_kwargs, test_tile=test_tile,
+                                 flip_x=flip_x, flip_y=flip_y)
+        depth.copy_(lr['depth'].reshape(H, W))
+        bgmap.copy_(lr['alphainv_last'].reshape(H, W))
+        frame_u8_cuda(lr['rgb_marched'].reshape(H, W, 3), render_video_flipy, k, out=lr_u8)
+        frame_u8_cuda(sr.permute(1, 2, 0), render_video_flipy, k, out=sr_u8)
+    return kdist.render_video_frames(render_into, len(render_poses), H, W, (*rot(s * H, s * W), 3), (*rot(H, W), 3),
+                                     next(model.parameters()).device, render_video_flipy, k, on_frame, group, dst)
+
+
+@torch.no_grad()
 def render_frame_4k_sharded(model, net_sr, H, W, K, c2w, ndc, render_kwargs, test_tile=510, out_u8=False,
                             flip_x=False, flip_y=False, group=None):
     """:func:`render_frame_4k` across the ranks of ``group`` (one process per GPU, scene and decoder

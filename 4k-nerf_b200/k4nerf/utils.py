@@ -254,20 +254,84 @@ def masked_quantiles_np(values, q=(5, 95)):
     s = _f32_of_keys(np.sort(_f32_keys(v)))
     out = []
     for t in qf:
-        vi = np.float64(n - 1) * t
-        if vi >= n - 1:
-            prev = nxt = n - 1
-            gamma = vi - np.float64(-1)
-        else:
-            prev = int(np.floor(vi))
-            nxt = prev + 1
-            gamma = vi - np.float64(prev)
-        a, b = s[prev], s[nxt]
-        with np.errstate(invalid='ignore'):                                 # inf - inf, as numpy's own
-            d = np.float64(np.float32(b - a))
-            r = np.float64(b) - d * (1 - gamma) if gamma >= 0.5 else np.float64(a) + d * gamma
+        prev, nxt, gamma = _np_indexes(n, t)
+        r = _np_lerp(s[prev], s[nxt], gamma)
         out.append(np.float64(np.nan) if np.isnan(v).any() else np.float64(r))
     return out[0], out[1]
+
+
+def _np_indexes(n, t):
+    """numpy's 'linear' order statistics of quantile fraction ``t`` among ``n`` values: ``(prev, next, gamma)``."""
+    vi = np.float64(n - 1) * t
+    if vi >= n - 1:
+        return n - 1, n - 1, vi - np.float64(-1)
+    prev = int(np.floor(vi))
+    return prev, prev + 1, vi - np.float64(prev)
+
+
+def _np_lerp(a, b, gamma):
+    """numpy's ``_lerp`` of two float32 order statistics: the difference in float32, the rest in float64."""
+    with np.errstate(invalid='ignore'):                                     # inf - inf, as numpy's own
+        d = np.float64(np.float32(b - a))
+        return np.float64(b) - d * (1 - gamma) if gamma >= 0.5 else np.float64(a) + d * gamma
+
+
+# The split select of k4_op_masked_quantiles_hist / _select restated: one share's int64 histogram per pass, and the
+# select of a summed histogram.  ``state`` is the per-pass state the C workspace holds (a dict, empty before pass 0).
+MQ_BINS, MQ_RANKS = 2048, 4
+MQ_HIST_LEN = MQ_RANKS * MQ_BINS + 2                  # include/k4nerf.h's K4_MASKED_QUANTILES_HIST_LEN
+_MQ_SHIFT, _MQ_NBINS = (21, 10, 0), (2048, 2048, 1024)
+
+
+def masked_quantiles_hist_np(p, values, state):
+    """Pass ``p``'s histogram of one share's selected float32 ``values`` (``depths_vis[bgmaps < 0.1]``), int64
+    ``[MQ_HIST_LEN]``: pass 0 the top 11 bits of every key, the count and the NaN count; passes 1 and 2 the next digit of
+    the keys under each distinct rank prefix, in the slot of the first rank with that prefix."""
+    v = np.asarray(values, dtype=np.float32).ravel()
+    k = _f32_keys(v).astype(np.int64)
+    hist = np.zeros(MQ_HIST_LEN, np.int64)
+    nb = _MQ_NBINS[p]
+    if p == 0:
+        hist[:nb] = np.bincount(k >> _MQ_SHIFT[0], minlength=nb)
+        hist[-2], hist[-1] = k.size, np.count_nonzero(np.isnan(v))
+        return hist
+    for r in range(MQ_RANKS):
+        if state['slot'][r] == r:
+            under = k[(k >> _MQ_SHIFT[p - 1]) == state['prefix'][r]]
+            hist[r * MQ_BINS:r * MQ_BINS + nb] = np.bincount((under >> _MQ_SHIFT[p]) & (nb - 1), minlength=nb)
+    return hist
+
+
+def masked_quantiles_select_np(p, hist, q, state):
+    """Pass ``p``'s select on the summed ``hist``: pass 0 turns the count into numpy's indexes, every pass narrows each
+    of the four ranks (prev / next of both quantiles) to one more digit, pass 2 returns ``(dmin, dmax, count)`` as
+    ``k4_op_masked_quantiles`` writes them (NaN quantiles for no or NaN values)."""
+    hist = np.asarray(hist, dtype=np.int64)
+    if p == 0:
+        n = int(hist[-2])
+        state.update(count=n, nans=int(hist[-1]), prefix=[0] * MQ_RANKS, slot=[0] * MQ_RANKS, rank=[], gamma=[])
+        for t in _quantile_fractions(q):
+            prev, nxt, gamma = _np_indexes(n, t) if n else (0, 0, 0.0)
+            state['rank'] += [prev, nxt]
+            state['gamma'].append(gamma)
+    nb = _MQ_NBINS[p]
+    for r in range(MQ_RANKS):
+        slot = state['slot'][r]
+        c = np.cumsum(hist[slot * MQ_BINS:slot * MQ_BINS + nb])
+        b = int(np.searchsorted(c, state['rank'][r], side='right'))           # the first bin whose prefix sum passes it
+        if b == nb:                                                           # no values at all: as the kernel, the last
+            b, below = nb - 1, state['rank'][r]
+        else:
+            below = int(c[b - 1]) if b else 0
+        state['prefix'][r] = (state['prefix'][r] << (10 if p == 2 else 11)) | b
+        state['rank'][r] -= below
+    state['slot'] = [state['prefix'].index(x) for x in state['prefix']]
+    if p < 2:
+        return None
+    n, v = state['count'], _f32_of_keys(np.array(state['prefix'], np.uint32))
+    out = [np.float64(np.nan) if n == 0 or state['nans'] else np.float64(_np_lerp(v[2 * j], v[2 * j + 1], state['gamma'][j]))
+           for j in range(2)]
+    return out[0], out[1], n
 
 
 def _flip_rot(frames, render_video_flipy, render_video_rot90):
@@ -295,6 +359,11 @@ def _depth_video_np(depths, bgmaps, q, render_video_flipy, render_video_rot90):
         raise ValueError(f'depths {depths.shape} and bgmaps {bgmaps.shape} differ')
     depths_vis = depths * (1 - bgmaps) + bgmaps
     dmin, dmax = masked_quantiles_np(depths_vis[bgmaps < 0.1], q)
+    return _colour_np(depths_vis, dmin, dmax, render_video_flipy, render_video_rot90), dmin, dmax
+
+
+def _colour_np(depths_vis, dmin, dmax, render_video_flipy, render_video_rot90):
+    """The rainbow frames of ``depths_vis`` under the range ``dmin, dmax`` (run_sr.py:1461-1463), flipped and rotated."""
     with np.errstate(divide='ignore', invalid='ignore'):
         x = 1 - np.clip((depths_vis - dmin) / (dmax - dmin), 0, 1)
         xa = x * 256
@@ -304,7 +373,7 @@ def _depth_video_np(depths, bgmaps, q, render_video_flipy, render_video_rot90):
     idx[bad] = 0
     frames = rainbow_lut_u8()[idx]
     frames[bad] = 0
-    return _flip_rot(frames, render_video_flipy, render_video_rot90), dmin, dmax
+    return _flip_rot(frames, render_video_flipy, render_video_rot90)
 
 
 def _strides3(t):
@@ -322,13 +391,7 @@ def _depth_video_cuda(depths, bgmaps, q, render_video_flipy, render_video_rot90)
     one 24-byte read of the range and count between them."""
     import ctypes as C
     from . import _lib
-    if not (_is_cuda(depths) and _is_cuda(bgmaps) and depths.device == bgmaps.device):
-        raise RuntimeError('depth_video_frames: depths and bgmaps must both be numpy / CPU or both on one CUDA device')
-    if depths.dtype != torch.float32 or bgmaps.dtype != torch.float32:
-        raise TypeError(f'depth_video_frames: float32 depths and bgmaps expected, got {depths.dtype} and {bgmaps.dtype}')
-    depths, bgmaps = _frames_of(depths.detach(), 'depths'), _frames_of(bgmaps.detach(), 'bgmaps')
-    if depths.shape != bgmaps.shape:
-        raise ValueError(f'depths {tuple(depths.shape)} and bgmaps {tuple(bgmaps.shape)} differ')
+    depths, bgmaps = _cuda_frames(depths, bgmaps)
     n, H, W = depths.shape
     qf = _quantile_fractions(q)
     k = int(render_video_rot90) % 4
@@ -345,12 +408,34 @@ def _depth_video_cuda(depths, bgmaps, q, render_video_flipy, render_video_rot90)
         if host[2] == 0:
             raise ValueError('the depth video needs at least one pixel with bgmap < 0.1')
         dmin, dmax = host[:2].view(np.float64)
-        out = torch.empty((n, W, H, 3) if k & 1 else (n, H, W, 3), dtype=torch.uint8, device=dev)
-        lut = np.ascontiguousarray(rainbow_lut_u8())
-        _cuda_call('k4_op_depth_video_u8', C.c_void_p(depths.data_ptr()), C.c_void_p(bgmaps.data_ptr()), n, H, W, sd, sb,
-                   C.c_void_p(res.data_ptr()), lut.ctypes.data_as(C.POINTER(C.c_uint8)), int(bool(render_video_flipy)), k,
-                   C.c_void_p(out.data_ptr()), stream)
+        out = _colour_cuda(depths, bgmaps, res, render_video_flipy, k, stream)
     return out, np.float64(dmin), np.float64(dmax)
+
+
+def _cuda_frames(depths, bgmaps):
+    """The checked ``[n, H, W]`` float32 views of CUDA ``depths`` / ``bgmaps`` on one device."""
+    if not (_is_cuda(depths) and _is_cuda(bgmaps) and depths.device == bgmaps.device):
+        raise RuntimeError('depth_video_frames: depths and bgmaps must both be numpy / CPU or both on one CUDA device')
+    if depths.dtype != torch.float32 or bgmaps.dtype != torch.float32:
+        raise TypeError(f'depth_video_frames: float32 depths and bgmaps expected, got {depths.dtype} and {bgmaps.dtype}')
+    depths, bgmaps = _frames_of(depths.detach(), 'depths'), _frames_of(bgmaps.detach(), 'bgmaps')
+    if depths.shape != bgmaps.shape:
+        raise ValueError(f'depths {tuple(depths.shape)} and bgmaps {tuple(bgmaps.shape)} differ')
+    return depths, bgmaps
+
+
+def _colour_cuda(depths, bgmaps, res, render_video_flipy, k, stream):
+    """``k4_op_depth_video_u8`` of ``[n, H, W]`` CUDA frames under the device range ``res[:2]`` (fp64 bits)."""
+    import ctypes as C
+    n, H, W = depths.shape
+    out = torch.empty((n, W, H, 3) if k & 1 else (n, H, W, 3), dtype=torch.uint8, device=depths.device)
+    if n == 0:
+        return out
+    lut = np.ascontiguousarray(rainbow_lut_u8())
+    _cuda_call('k4_op_depth_video_u8', C.c_void_p(depths.data_ptr()), C.c_void_p(bgmaps.data_ptr()), n, H, W,
+               _strides3(depths), _strides3(bgmaps), C.c_void_p(res.data_ptr()), lut.ctypes.data_as(C.POINTER(C.c_uint8)),
+               int(bool(render_video_flipy)), k, C.c_void_p(out.data_ptr()), stream)
+    return out
 
 
 def depth_video_frames(depths, bgmaps, q=(5, 95), render_video_flipy=False, render_video_rot90=0, return_range=False):
@@ -374,6 +459,75 @@ def depth_video_frames(depths, bgmaps, q=(5, 95), render_video_flipy=False, rend
         out, dmin, dmax = _depth_video_cuda(depths, bgmaps, q, render_video_flipy, render_video_rot90)
     else:
         out, dmin, dmax = _depth_video_np(depths, bgmaps, q, render_video_flipy, render_video_rot90)
+    return (out, (dmin, dmax)) if return_range else out
+
+
+def _depth_video_sharded_cuda(depths, bgmaps, q, render_video_flipy, k, all_reduce):
+    """The split passes (``k4_op_masked_quantiles_hist`` / ``_select``) with ``all_reduce`` summing each pass's
+    histogram over the shares, then ``k4_op_depth_video_u8`` of this share's frames; one 24-byte read of the range."""
+    import ctypes as C
+    from . import _lib
+    depths, bgmaps = _cuda_frames(depths, bgmaps)
+    n, H, W = depths.shape
+    dev = depths.device
+    with torch.cuda.device(dev):
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        ws = torch.empty(_lib.lib.k4_op_masked_quantiles_pass_workspace_bytes(), dtype=torch.uint8, device=dev)
+        hist = torch.empty(_lib.K4_MASKED_QUANTILES_HIST_LEN, dtype=torch.int64, device=dev)
+        res = torch.empty(3, dtype=torch.int64, device=dev)              # dmin, dmax (fp64 bits), count
+        sd, sb, q = _strides3(depths), _strides3(bgmaps), (C.c_double * 2)(*_quantile_fractions(q).tolist())
+        for p in range(3):
+            hist.zero_()
+            _cuda_call('k4_op_masked_quantiles_hist', p, C.c_void_p(depths.data_ptr()), C.c_void_p(bgmaps.data_ptr()),
+                       n, H, W, sd, sb, C.c_void_p(hist.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(), stream)
+            all_reduce(hist)
+            _cuda_call('k4_op_masked_quantiles_select', p, C.c_void_p(hist.data_ptr()), q, C.c_void_p(res.data_ptr()),
+                       C.c_void_p(res.data_ptr() + 16), C.c_void_p(ws.data_ptr()), ws.numel(), stream)
+        host = res.cpu().numpy()
+        if host[2] == 0:
+            raise ValueError('the depth video needs at least one pixel with bgmap < 0.1')
+        dmin, dmax = host[:2].view(np.float64)
+        out = _colour_cuda(depths, bgmaps, res, render_video_flipy, k, stream)
+    return out, np.float64(dmin), np.float64(dmax)
+
+
+def _depth_video_sharded_np(depths, bgmaps, q, render_video_flipy, k, all_reduce):
+    """The numpy restatement of the split passes (``masked_quantiles_hist_np`` / ``_select_np``), then the colours."""
+    depths = _frames_of(np.asarray(depths, dtype=np.float32), 'depths')
+    bgmaps = _frames_of(np.asarray(bgmaps, dtype=np.float32), 'bgmaps')
+    if depths.shape != bgmaps.shape:
+        raise ValueError(f'depths {depths.shape} and bgmaps {bgmaps.shape} differ')
+    depths_vis = depths * (1 - bgmaps) + bgmaps
+    values, state = depths_vis[bgmaps < 0.1], {}
+    for p in range(3):
+        hist = torch.from_numpy(masked_quantiles_hist_np(p, values, state))
+        all_reduce(hist)
+        res = masked_quantiles_select_np(p, hist.numpy(), q, state)
+    dmin, dmax, count = res
+    if count == 0:
+        raise ValueError('the depth video needs at least one pixel with bgmap < 0.1')
+    return _colour_np(depths_vis, dmin, dmax, render_video_flipy, k), dmin, dmax
+
+
+def depth_video_frames_sharded(depths, bgmaps, q=(5, 95), render_video_flipy=False, render_video_rot90=0, group=None,
+                               return_range=False):
+    """:func:`depth_video_frames` of a video whose frames are spread over the ranks of ``group``: each rank passes its
+    own ``[n_r, H, W]`` (or ``[n_r, H, W, 1]``) depth and bgmap frames, ``n_r`` may be 0, and gets its own frames'
+    colours, ``[n_r, H', W', 3]`` uint8, under the range of ALL the ranks' frames.  That range is exact: each of the
+    select's three passes builds the integer histogram of the rank's own keys (``k4_op_masked_quantiles_hist``), one
+    ``all_reduce(SUM)`` adds them, and every rank selects on the sum (``k4_op_masked_quantiles_select``), so all ranks
+    reach the same order statistics as ``np.percentile`` over every frame, bit for bit.  CUDA tensors run on the GPU
+    (a gloo group takes the histogram through the host); numpy arrays and CPU tensors take the numpy restatement and
+    give numpy arrays.  On a group of one rank (or without a process group) the result is :func:`depth_video_frames`'.
+    No selected pixel on any rank raises ``ValueError`` on every rank.  Collective: every rank of ``group`` calls it."""
+    from . import dist as kdist
+    _quantile_fractions(q)                                  # a bad q raises before any collective
+    k = int(render_video_rot90) % 4
+    all_reduce = lambda t: kdist.all_reduce_sum(t, group)
+    if _is_cuda(depths) or _is_cuda(bgmaps):
+        out, dmin, dmax = _depth_video_sharded_cuda(depths, bgmaps, q, render_video_flipy, k, all_reduce)
+    else:
+        out, dmin, dmax = _depth_video_sharded_np(depths, bgmaps, q, render_video_flipy, k, all_reduce)
     return (out, (dmin, dmax)) if return_range else out
 
 

@@ -583,6 +583,37 @@ K4_API int k4_op_depth_video_u8(const float* d_depth, const float* d_bgmap, int6
 K4_API int k4_op_frame_u8(const float* d_rgb, int64_t H, int64_t W, const int64_t strides[3], int32_t flip_y, int32_t rot90,
                           uint8_t* d_out, k4_stream_t stream);
 
+/* The passes of k4_op_masked_quantiles one by one, for frames spread over several GPUs (or any set of shares).  The
+ * select's three passes each read a histogram of integer counts, and integer counts add exactly, so per pass p = 0, 1, 2:
+ *   1. every share zeroes an int64 histogram of K4_MASKED_QUANTILES_HIST_LEN entries and adds its frames into it with
+ *      k4_op_masked_quantiles_hist(p, ...);
+ *   2. the caller sums the shares' histograms element by element (e.g. one all-reduce);
+ *   3. every share runs k4_op_masked_quantiles_select(p, ...) on the sum.
+ * Every share then holds the same state for pass p + 1, and after pass 2 d_quantiles and d_count are bit for bit
+ * k4_op_masked_quantiles' over all the shares' frames, in the same layout.  The histogram's last two entries hold the
+ * count and the NaN count of pass 0 (zero in passes 1 and 2).  The workspace holds the per-pass state:
+ * k4_op_masked_quantiles_pass_workspace_bytes() bytes, 16-byte aligned, kept by the caller from pass 0 to pass 2; it needs
+ * no initialisation.
+ * k4_op_masked_quantiles_hist ADDS into d_hist (int64 counts, 8-byte aligned).  n == 0 (a share without frames) is valid
+ * and launches nothing; d_depth and d_bgmap may then be NULL.  The select takes the same h_q on every pass (pass 0 reads
+ * it) and writes d_quantiles / d_count in pass 2.  Caller's stream, no host sync.
+ * A pass outside 0 .. 2, a NULL pointer, n below 0, H or W below 1, n * H above 2^31 - 1, a quantile outside [0, 1] or
+ * NaN, or a misaligned pointer: K4_ERR_INVALID_ARG; a workspace smaller than the size: K4_ERR_WORKSPACE. */
+#define K4_MASKED_QUANTILES_HIST_LEN (4 * 2048 + 2)
+/* Replaces: np.percentile(depths_vis[bgmaps < 0.1], q=[5, 95]) (run_sr.py:1460) over frames spread over GPUs -- the
+ * per-pass state of k4_op_masked_quantiles_hist / _select. */
+K4_API size_t k4_op_masked_quantiles_pass_workspace_bytes(void);
+/* Replaces: np.percentile(depths_vis[bgmaps < 0.1], q=[5, 95]) (run_sr.py:1459-1460) over frames spread over GPUs --
+ * one share's histogram of pass `pass`. */
+K4_API int k4_op_masked_quantiles_hist(int32_t pass, const float* d_depth, const float* d_bgmap, int64_t n, int64_t H,
+                                       int64_t W, const int64_t depth_strides[3], const int64_t bgmap_strides[3],
+                                       int64_t* d_hist, const void* d_workspace, size_t workspace_bytes,
+                                       k4_stream_t stream);
+/* Replaces: np.percentile(depths_vis[bgmaps < 0.1], q=[5, 95]) (run_sr.py:1460) over frames spread over GPUs -- the
+ * select of pass `pass` on the summed histogram. */
+K4_API int k4_op_masked_quantiles_select(int32_t pass, const int64_t* d_hist, const double h_q[2], double* d_quantiles,
+                                         int64_t* d_count, void* d_workspace, size_t workspace_bytes, k4_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Testing.  Entry points for the test suite, not for renderers: they replace no reference interface and may change
  * with the kernels they expose.
