@@ -296,7 +296,7 @@ extern "C" int k4_scene_create(const k4_scene_desc* d, k4_stream_t stream, k4_sc
                      d->kind == K4_KIND_DVGO ? (d->rgbnet_direct != 0) : 1, d->rgbnet_depth, want_cfg)
         : nullptr;
     if (wcfg && round_up(wcfg->C, 4) > v.Cpad) v.Cpad = round_up(wcfg->C, 4);
-    v.tc_cfg = -1; v.tc_exact = 0;
+    v.tc_cfg = -1;
     v.mX = d->mask_size[0]; v.mY = d->mask_size[1]; v.mZ = d->mask_size[2];
     for (int a = 0; a < 3; ++a) {
         v.xyz_min[a] = d->xyz_min[a]; v.xyz_max[a] = d->xyz_max[a];
@@ -453,7 +453,6 @@ extern "C" int k4_scene_create(const k4_scene_desc* d, k4_stream_t stream, k4_sc
                 pack_tc_ones_kernel<<<8, 256, 0, s>>>(blob + BL.off_ones);
                 K4_CTRY(cudaGetLastError());
                 v.tc_blob = blob; v.tc_kpad = kpad; v.tc_width = w; v.tc_cfg = c.id; v.tc_colmap = d_colmap;
-                v.tc_exact = (c.C == v.C && c.vpe == v.viewpe && c.spe == v.spape && c.W == v.width) ? 1 : 0;
             }
         }
     }
@@ -538,10 +537,8 @@ static int render_impl(const k4_scene* sc, const k4_render_args* a,
     rp.ray_stats = out->d_ray_stats; rp.t_minmax = out->d_t_minmax; rp.counters = out->d_counters;
     rp.tile_counter = reinterpret_cast<unsigned int*>(d_workspace);
     K4_CUDA_TRY(cudaMemsetAsync(d_workspace, 0, 16, s));
-    if ((a->mlp_mode == K4_MLP_TCGEN05 || a->mlp_mode == K4_MLP_TCGEN05_WS) && v.depth > 0) {
-        if (a->mlp_mode == K4_MLP_TCGEN05) return k4_tc_supported(v) ? k4_launch_march_tc(sc, rp, s) : K4_ERR_UNSUPPORTED;
+    if ((a->mlp_mode == K4_MLP_TCGEN05 || a->mlp_mode == K4_MLP_TCGEN05_WS) && v.depth > 0)   // K4_MLP_TCGEN05: an alias
         return k4_ws_supported(v) ? k4_launch_march_ws(sc, rp, s, phases, max_ctas, n_ctas) : K4_ERR_UNSUPPORTED;
-    }
     return k4_launch_march(sc, rp, a->mlp_mode, s);
 }
 

@@ -42,7 +42,6 @@ struct K4Dev {
     const unsigned char* tc_blob;
     int tc_kpad, tc_width;
     int tc_cfg;                   // id of the K4_WS_CFG_LIST entry (k4_ws_cfgs.h) the blob is packed for, -1: none
-    int tc_exact;                 // the model's own shape equals that entry's (k4_march_tc.cu only runs exact shapes)
     // empty-space skipping (k4_march_common.cuh skip_steps): Chebyshev distance field over K4_SKIP_B^3-voxel cells of
     // the occupancy mask, in cells: 0 = the cell holds an occupied voxel, d = every cell within d-1 is empty
     const uint8_t* skip;          // [cX,cY,cZ] or nullptr (skipping off)
@@ -131,12 +130,10 @@ void k4_set_cuda_error(cudaError_t e, const char* where);
 
 // launchers
 int k4_launch_march(const k4_scene* sc, const K4RenderParams& rp, int mlp_mode, cudaStream_t st);
-int k4_launch_march_tc(const k4_scene* sc, K4RenderParams rp, cudaStream_t st);   // K4_ERR_UNSUPPORTED if the shape has no wgmma build
-bool k4_tc_supported(const K4Dev& v);
 bool k4_ws_supported(const K4Dev& v);
 // k4_testing_ws_row_layout: the compile-time row layout of K4_WS_CFG_LIST entry `id` (k4_march_ws.cu)
 int k4_ws_row_layout(int id, int32_t out[4]);
-// warp-specialised variant (same shapes).  phases != NULL runs the profiled kernel (k4_testing_march_phases), which
+// the warp-specialised wgmma marcher; K4_ERR_UNSUPPORTED if the shape has no wgmma build.  phases != NULL runs the profiled kernel (k4_testing_march_phases), which
 // writes the phase counters of at most max_ctas CTAs there; *n_ctas (may be NULL) receives the CTA count
 int k4_launch_march_ws(const k4_scene* sc, K4RenderParams rp, cudaStream_t st, unsigned long long* phases = nullptr,
                        int max_ctas = 0, int* n_ctas = nullptr);

@@ -16,8 +16,8 @@
 // tensor cores (f16 modes, k4_march_mma.cuh).
 //
 // The per-ray geometry, the marching step up to the shade decision and the ray's results are in
-// k4_march_ray.cuh, the one copy this kernel shares with k4_march_tc.cu and k4_march_ws.cu (its
-// header gives the floating-point shape that keeps the geometry bit-identical to the reference).
+// k4_march_ray.cuh, the one copy this kernel shares with k4_march_ws.cu (its header gives the
+// floating-point shape that keeps the geometry bit-identical to the reference).
 #include "k4_internal.cuh"
 #include "k4_march_common.cuh"
 #include "k4_march_ray.cuh"

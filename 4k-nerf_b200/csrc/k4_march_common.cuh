@@ -128,7 +128,7 @@ __device__ __forceinline__ void interp_k0(const K4Dev& s, const float w[8], cons
     }
 }
 
-// The same gather for a copy of exactly NQ channel quads per voxel (s.Cpad == 4 * NQ, the wgmma marchers' configs):
+// The same gather for a copy of exactly NQ channel quads per voxel (s.Cpad == 4 * NQ, the wgmma marcher's configs):
 // no run-time channel count and no branch per quad, the corner rows addressed once with the quads at immediate offsets,
 // loads issued KR corners (all their quads) at a time.  ptxas still interleaves the loads of later corners with the
 // FMAs of earlier ones; what this saves is the per-quad branches and address arithmetic.  With 4 quads the unbranched

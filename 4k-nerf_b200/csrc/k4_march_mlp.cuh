@@ -1,4 +1,4 @@
-// k4_march_mlp.cuh -- the rgbnet of the fused marchers (k4_march_tc.cu, k4_march_ws.cu) on Hopper warpgroup MMAs.
+// k4_march_mlp.cuh -- the rgbnet of the warp-specialised marcher (k4_march_ws.cu) on Hopper warpgroup MMAs.
 //
 // One warpgroup runs a batch of 128 queued sample rows through the three layers, 64 rows (one wgmma M) at a time:
 //   L1  acc[64 x W] = A(ring tile, smem) * W1(smem) + bias             wgmma SS, fp32 accumulate in registers

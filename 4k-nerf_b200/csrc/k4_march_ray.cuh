@@ -1,5 +1,5 @@
-// k4_march_ray.cuh -- what one thread does for one ray in every fused marcher (k4_march.cu, k4_march_tc.cu,
-// k4_march_ws.cu), independent of how the surviving samples are shaded: the per-ray geometry, one marching step up to
+// k4_march_ray.cuh -- what one thread does for one ray in both fused marchers (k4_march.cu, k4_march_ws.cu),
+// independent of how the surviving samples are shaded: the per-ray geometry, one marching step up to
 // the shade / skip decision, and the per-ray and per-warp results.  The one copy of
 //   sample_pts_on_rays / sample_ndc_pts_on_rays   lib/cuda/render_utils_kernel.cu:12-79,167-194,245-270
 //   maskcache_lookup                               lib/cuda/render_utils_kernel.cu:373-392

@@ -12,8 +12,7 @@ K4_ACT_RELU, K4_ACT_GAUSS, K4_ACT_LKRELU = 0, 1, 2
 K4_MAX_MLP_LAYERS = 8
 K4_MAX_PEERS = 8
 K4_MASKED_QUANTILES_HIST_LEN = 4 * 2048 + 2
-MLP_MODES = {'fp32': K4_MLP_FP32, 'f16': K4_MLP_F16, 'f16x3': K4_MLP_F16X3, 'tcgen05': K4_MLP_TCGEN05,
-             'tc': K4_MLP_TCGEN05, 'ws': K4_MLP_TCGEN05_WS}
+MLP_MODES = {'fp32': K4_MLP_FP32, 'f16': K4_MLP_F16, 'f16x3': K4_MLP_F16X3, 'ws': K4_MLP_TCGEN05_WS}
 
 
 class SceneDesc(C.Structure):

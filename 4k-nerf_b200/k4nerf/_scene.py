@@ -172,7 +172,9 @@ class FusedRenderMixin:
 
     def resolve_mlp_mode(self, mode):
         """'auto' -> the fastest mode built for this model's shape (every mode is checked against the fp32
-        oracle by tests/test_gpu_marcher.py)."""
+        oracle by tests/test_gpu_marcher.py).  'tc' / 'tcgen05' name the wgmma marcher, 'ws'."""
+        if mode in ('tc', 'tcgen05'):
+            return 'ws'
         if mode != 'auto':
             return mode
         if not linear_layers(self.rgbnet):

@@ -121,11 +121,6 @@ class DirectContractedVoxGO(FusedRenderMixin, GridMaintenanceMixin, CoarseStageM
             return forward_samples(self, rays_o, rays_d, viewdirs, global_step=global_step, is_train=is_train, **render_kwargs)
         return super().forward(rays_o, rays_d, viewdirs, global_step=global_step, **render_kwargs)
 
-    def resolve_mlp_mode(self, mode):
-        if mode == 'tc':
-            return 'ws'        # the contracted front-end is built into the warp-specialised kernel only
-        return super().resolve_mlp_mode(mode)
-
     def _scene_extra(self):
         bufs = [self.act_shift, self.scene_center, self.scene_radius]
         act, center, radius = cached_host(self, 'scene_host', bufs, lambda: (

@@ -54,8 +54,8 @@ enum { K4_KIND_DVGO = 0,                   /* DirectVoxGO,            lib/dvgo.p
 enum { K4_MLP_FP32 = 0,                    /* fp32 FFMA, sequential accumulation (exact mode)   */
        K4_MLP_F16 = 1,                     /* tensor cores, fp16 operands, fp32 accumulate       */
        K4_MLP_F16X3 = 2,                   /* tensor cores, error-compensated 3-term fp16 split  */
-       K4_MLP_TCGEN05 = 3,                 /* wgmma, fp16 operands (warpgroup-wide batches)      */
-       K4_MLP_TCGEN05_WS = 4 };            /* same, MLP in its own warpgroup (warp-specialised)  */
+       K4_MLP_TCGEN05 = 3,                 /* alias of K4_MLP_TCGEN05_WS, kept for compatibility */
+       K4_MLP_TCGEN05_WS = 4 };            /* wgmma, fp16 operands, MLP in its own warpgroups    */
 
 /* The colour MLP's hidden activation (DirectMPIGO's fine_model_and_render.act_type, lib/dmpigo.py:89-95): the
  * module after every hidden nn.Linear.  DirectVoxGO and DirectContractedVoxGO always use K4_ACT_RELU.
@@ -787,7 +787,8 @@ K4_API int k4_testing_srnet_forward_upto(const k4_srnet* net, const float* d_x, 
  *   diffuse logits k0[0:3] of a DirectVoxGO model with rgbnet_direct=False, NULL for every other model.  d_w [n]: sample
  *   weights.  d_owner [n]: the row's owner inside its group.
  *   Rows form groups of G consecutive rows (*group_rows receives G; the last group may be partial):
- *     K4_MLP_TCGEN05 / _WS  G = 128: one warpgroup batch of mlp_batch_wgmma; the rows are written into a ring tile through
+ *     K4_MLP_TCGEN05_WS     G = 128 (also for its alias K4_MLP_TCGEN05): one warpgroup batch of mlp_batch_wgmma; the
+ *                           rows are written into a ring tile through
  *                           the column map of the scene's K4_WS_CFG_LIST entry, as fp16 with saturation
  *     K4_MLP_F16 / _F16X3   G = 32: one warp's MmaWarpCtx, rows appended as the marcher appends them, flushed at 32 rows
  *                           and at the end of the group

@@ -22,13 +22,13 @@ end on a 128-row boundary all carry the empty batch.
 
 A ray tile is four warps of 32 rays.  Laid out in linear order, tile t is rays [128 t, 128 t + 128) and its warp w
 rays [128 t + 32 w, ..); laid out in image order (16 x 8 pixel blocks), the tile is block t and its warp w the 8 x 4 block
-the 'ws' / 'tc' marchers give warp w -- which is also the mma.sync marchers' warp tile.  So one composition pins the
-rows of every 'ws' / 'tc' tile and of every mma.sync warp tile in both orders.
+the 'ws' marcher gives warp w -- which is also the mma.sync marchers' warp tile.  So one composition pins the
+rows of every 'ws' tile and of every mma.sync warp tile in both orders.
 
-Batch counts (counters[3]) with K4_NO_SKIP=1, derived from k4_march_ws.cu / k4_march_tc.cu / k4_march_mma.cuh:
-  * 'tc': a batch whenever 128 rows are pending at a rendezvous, and one for a partial remainder: sum ceil(n_t / 128).
-  * 'ws': the same cut, plus an empty batch carrying only WgCtl::last for a tile whose rows end on a 128-row boundary
-    while one of its rays still marches: the batch of the last 128 rows went out without `last` (tile_open).
+Batch counts (counters[3]) with K4_NO_SKIP=1, derived from k4_march_ws.cu / k4_march_mma.cuh:
+  * 'ws': a batch whenever 128 rows are pending at a rendezvous, and one for a partial remainder: sum ceil(n_t / 128);
+    plus an empty batch carrying only WgCtl::last for a tile whose rows end on a 128-row boundary while one of its rays
+    still marches: the batch of the last 128 rows went out without `last` (tile_open).
   * f16 / f16x3: each warp flushes every 32 rows and once for a remainder: sum over warp tiles of ceil(n_w / 32).
 The warps of a 'ws' group do not march in lockstep: between rendezvous each takes up to TC_ROUND steps and stops early
 once 128 rows are pending, so one warp may run ahead of another, by more steps over a long tile.  Whether a ray is live
@@ -59,11 +59,11 @@ KWS = {'dvgo': dict(scenes.RENDER_KW_DVGO, near=0.1, bg=0.37),
        'dmpigo': dict(scenes.RENDER_KW_MPI, stepsize=0.5, bg=0.37),
        'dcvgo': dict(scenes.RENDER_KW_DCVGO, bg=0.37)}
 # configuration id (csrc/k4_ws_cfgs.h) -> (kind, rgbnet shape):
-#   1  DirectVoxGO, the 'tc' shape and 'ws'
+#   1  DirectVoxGO, the fine stage of configs/default.py
 #   2  DirectVoxGO, 'ws' with the ones-tile MMA: its 15 inputs fill layer 1's 16 columns, no padding column for the bias
-#   6  DirectMPIGO, the other 'tc' shape and 'ws'
+#   6  DirectMPIGO, the LLFF shape
 #   7  DirectMPIGO, 'ws' writing the bias word from the row store (BIAS_STORED)
-#  10  DirectContractedVoxGO, 'ws' ('tc' runs on the 'ws' kernel there)
+#  10  DirectContractedVoxGO
 CFGS = {1: ('dvgo', dict(rgbnet_dim=12, rgbnet_depth=3, rgbnet_width=128, viewbase_pe=4)),
         2: ('dvgo', dict(rgbnet_dim=12, rgbnet_depth=3, rgbnet_width=64, viewbase_pe=0)),
         6: ('dmpigo', dict(rgbnet_dim=9, rgbnet_depth=3, rgbnet_width=64, viewbase_pe=0, spatial_pe=0)),
@@ -133,7 +133,7 @@ def kind_of(cfg):
 
 def modes_of(st):
     shp = types_ns(st)
-    return tuple(m for m in ('fp32', 'f16', 'f16x3', 'tc', 'ws') if m == 'fp32' or supports(shp.spec, m))
+    return tuple(m for m in ('fp32', 'f16', 'f16x3', 'ws') if m == 'fp32' or supports(shp.spec, m))
 
 
 def spacing(kind):
@@ -204,7 +204,7 @@ def marching(specs, kind, n, rng):
 
 
 def ws_tiles(kind, seed=0):
-    """[(name, n_t, empty last batch expected, tile)] for the 'ws' / 'tc' targets."""
+    """[(name, n_t, empty last batch expected, tile)] for the 'ws' targets."""
     rng = np.random.default_rng(seed)
     base = 'end' if kind != 'dcvgo' else 'march'
     out = []
@@ -293,7 +293,7 @@ def n_steps_of(st, ref, N):
 
 def replay(trace, n_steps, hw):
     """Per-tile rows and expected batch counts from the oracle's trace (module docstring).  n_steps: every ray's step
-    count (n_steps_of).  Returns dict(n_t, empty, n_w, tc, ws, ws_lo, ws_hi, f16) with n_t / empty per 'ws' tile and n_w
+    count (n_steps_of).  Returns dict(n_t, empty, n_w, ws, ws_lo, ws_hi, f16) with n_t / empty per 'ws' tile and n_w
     per warp tile."""
     N = n_steps.shape[0]
     rid = trace['ray_id'].long().numpy()
@@ -311,7 +311,7 @@ def replay(trace, n_steps, hw):
     mt = tile_ids(N, hw, 8, 4)
     n_w = np.bincount(mt[rid], minlength=int(mt.max()) + 1)
     full = int(sum(-(-int(n) // 128) for n in n_t))
-    return dict(n_t=n_t, empty=empty, n_w=n_w, tc=full, ws=full + int(empty.sum()),
+    return dict(n_t=n_t, empty=empty, n_w=n_w, ws=full + int(empty.sum()),
                 ws_lo=full, ws_hi=full + int(((n_t > 0) & (n_t % 128 == 0)).sum()),
                 f16=int(sum(-(-int(n) // 32) for n in n_w)))
 

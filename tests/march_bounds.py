@@ -23,13 +23,11 @@ def dim0_of(kind, c, vpe, spe, direct):
 def supports(spec, mode):
     """The modes a model shape has a build for.  mma.sync (f16 / f16x3): widths 64 / 128 and up to 64 inputs; f16x3
     keeps two weight parts and two rows per ring slot in shared memory, which do not fit a block (227 KB) at width 128
-    with more than 48 inputs.  tc: the two shapes k4_march_tc.cu is instantiated for.  fp32 and ws: every shape here."""
+    with more than 48 inputs.  fp32 and ws: every shape here."""
     name, kind, c, vpe, spe, w, direct, cid = spec
     kpad = (dim0_of(kind, c, vpe, spe, direct) + 15) // 16 * 16
     if mode in ('f16', 'f16x3'):
         return kpad <= 64 and w in (64, 128) and not (mode == 'f16x3' and w == 128 and kpad > 48)
-    if mode == 'tc':
-        return (kind, c, vpe, spe, w, direct) in (('cfgA', 12, 4, 0, 128, 1), ('cfgB', 9, 0, 0, 64, 1))
     return True
 
 
@@ -116,7 +114,7 @@ def true_logit_bound(mode, m, x, diff, D0=None):
     |v - fp16(v)| <= 2^-11 |v| + 2^-25; the wgmma bias hi + lo misses at most 2^-22 |b| + 2^-25."""
     if mode in ('fp32', 'f16x3'):
         return logit_bound(mode, m, x, diff, D0)
-    wg = mode in ('ws', 'tc')
+    wg = mode == 'ws'
     ks = [m.kpad_cfg, m.w_cfg, m.w_cfg] if wg else [m.kpad_mma, m.width, m.width]
     a, D = x, (np.zeros_like(x) if D0 is None else D0)
     for i, (W, b) in enumerate(m.layers):

@@ -216,10 +216,10 @@ def _act_step(z, E, act, a, tc):
 def act_logit_bound(mode, m, x, diff, act, a=A_GAUSS, D0=None, true=False):
     """march_bounds.logit_bound (true=False: f16 / ws held to the fp16-quantised model) or true_logit_bound (true=True:
     every mode held to the unquantised fp64 model) with the hidden activation `act`.  Returns (logits [n, 3], bound)."""
-    wg = mode in ('ws', 'tc')
+    wg = mode == 'ws'
     tc = mode != 'fp32'
     layers = m.layers
-    if mode in ('f16', 'ws', 'tc') and not true:
+    if mode in ('f16', 'ws') and not true:
         h = f16(np.clip(x, -65504, 65504))
         D = np.zeros_like(h)
         ks = [m.kpad_cfg, m.w_cfg, m.w_cfg] if wg else [m.kpad_mma, m.width, m.width]

@@ -1,9 +1,9 @@
 """GPU: how the marchers cut their shaded samples into MLP batches, on scenes whose per-tile row counts are chosen
-(march_batches.py): tiles that end before, on and after every 128-row ('ws' / 'tc') and 32-row (f16 / f16x3) boundary,
+(march_batches.py): tiles that end before, on and after every 128-row ('ws') and 32-row (f16 / f16x3) boundary,
 a tile ending on a boundary while a ray still marches ('ws' sends an empty batch that only carries `last`), a step that
 appends 128 rows with 50 pending, and a ring that wraps many times -- one tile per marcher group, and a frame of 24
 times as many tiles, so the groups carry their FULL / DONE phases from tile to tile.  Configurations 1 and 2
-(DirectVoxGO; 'tc' and the ones-tile 'ws' build), 6 and 7 (DirectMPIGO; the second 'tc' shape and the 'ws' build that
+(DirectVoxGO; the fine-stage shape and the ones-tile build), 6 and 7 (DirectMPIGO; the LLFF shape and the build that
 stores the bias word with each row) and 10 (DirectContractedVoxGO).
 
 Per render (every mode the shape has, image and linear order, empty-space skipping on and off):
@@ -52,9 +52,7 @@ def run(st, ms, rays, label):
             reps[order] = mb.replay(trace, n_steps, order)
         rep = reps[order]
         got = int(o['counters'][3])
-        if mode == 'tc':
-            lo = hi = rep['tc']
-        elif mode in ('f16', 'f16x3'):
+        if mode in ('f16', 'f16x3'):
             lo = hi = rep['f16']
         elif skip and st['kind'] != 'dcvgo':
             lo, hi = rep['ws_lo'], rep['ws_hi']
@@ -74,7 +72,7 @@ CFGS = sorted(mb.CFGS)
 
 
 @pytest.mark.parametrize('cfg', CFGS)
-def test_batches_at_their_boundaries(cuda_device, monkeypatch, cfg):
+def test_batch_counts_at_their_boundaries(cuda_device, monkeypatch, cfg):
     """One tile per marcher group: every target tile laid out in linear order and, as 16 x 8 blocks, in image order."""
     st = mb.scene(cfg)
     kind = mb.kind_of(cfg)
@@ -84,7 +82,7 @@ def test_batches_at_their_boundaries(cuda_device, monkeypatch, cfg):
 
 
 @pytest.mark.parametrize('cfg', CFGS)
-def test_batches_across_tiles(cuda_device, monkeypatch, cfg):
+def test_batch_counts_across_tiles(cuda_device, monkeypatch, cfg):
     """The target tiles 24 times over (in image order 24 blocks wide) on 2 x 132 marcher groups: every group takes
     several tiles and runs its FULL / DONE phases on across them, among them tiles after an empty last batch."""
     st = mb.scene(cfg)

@@ -14,7 +14,7 @@ and with empty-space skipping on and off.  Checks per ray:
     Skipping on and off must give identical outputs and ray_stats.
   * values, fp32 mode against a float64 recomposition of the same ray from the oracle's trace (fp64_reference): rgb,
     depth and alphainv_last within a bound built from that ray's own samples.
-  * tensor-core modes against fp32 mode with the bound of test_gpu_march_mlp.test_every_mode_against_fp32_per_ray.
+  * tensor-core modes against fp32 mode with the bound of test_gpu_march_mlp.check_per_ray_against_fp32.
 
 Error model of the recomposition (u = 2^-24):
   * density: the marcher's trilinear sum (k4_march_common.cuh) and the oracle's CPU grid_sample use the same fp32 corner
@@ -60,8 +60,8 @@ BOX_A = ([-0.7, -1.3, -0.2], [1.1, 0.4, 0.9])                 # off-centre, non-
 BOX_B = ([-0.75, -1.25, -0.5], [1.25, 0.5, 0.875])            # off-centre, with dyadic extents: exact mask scale / shift
 FG_BOX = ([-0.6, -1.2, -0.3], [1.0, 0.5, 0.9])                # DCVGO foreground: centre (0.2, -0.35, 0.3), radii .8 .85 .6
 MPI_BOX = ([-1.3, -1.9, -1.0], [1.7, 1.2, 0.9])
-RGBNET = dict(rgbnet_dim=12, rgbnet_depth=3, rgbnet_width=128, viewbase_pe=4)     # tc configuration 1 (exact shape)
-MPI_RGBNET = dict(rgbnet_dim=9, rgbnet_depth=3, rgbnet_width=64, viewbase_pe=0, spatial_pe=0)   # tc configuration 6
+RGBNET = dict(rgbnet_dim=12, rgbnet_depth=3, rgbnet_width=128, viewbase_pe=4)     # wgmma configuration 1 (exact shape)
+MPI_RGBNET = dict(rgbnet_dim=9, rgbnet_depth=3, rgbnet_width=64, viewbase_pe=0, spatial_pe=0)   # wgmma configuration 6
 
 
 def _num_voxels(box, dims):
@@ -226,7 +226,7 @@ def modes_of(st):
         return ('fp32', 'f16', 'f16x3', 'ws', 'auto')
     if st['rgbnet'] is None:
         return ('fp32', 'auto')
-    return ('fp32', 'f16', 'f16x3', 'tc', 'ws')
+    return ('fp32', 'f16', 'f16x3', 'ws')
 
 
 def render_all(ms, ro, rd, vd, kw, hw, modes):
@@ -422,7 +422,7 @@ def check_values(out, ref64, label, ratios):
 
 
 def tc_bounds(st, trace, ref64, rgb_f, modes):
-    """{mode: [N, 3]}: test_every_mode_against_fp32_per_ray's bound on |rgb_mode - rgb_fp32| per ray, with the weights
+    """{mode: [N, 3]}: check_per_ray_against_fp32's bound on |rgb_mode - rgb_fp32| per ray, with the weights
     bounded by the recomposition's w_hi; rgb_f is fp32 mode's colour."""
     shp = types_ns(st)
     x = trace['rgb_feat'].double().numpy()
@@ -448,7 +448,7 @@ def tc_bounds(st, trace, ref64, rgb_f, modes):
 
 
 def check_tc_against_fp32(fp, outs, st, trace, ref64, skip_rays, label, ratios):
-    """test_every_mode_against_fp32_per_ray's bound (tc_bounds)."""
+    """check_per_ray_against_fp32's bound (tc_bounds)."""
     if st['rgbnet'] is None:
         return
     N = fp['rgb_marched'].shape[0]

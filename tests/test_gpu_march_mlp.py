@@ -1,16 +1,15 @@
 """GPU: the marchers' colour MLP (rgbnet) sample by sample, and per ray, against float64 references.
 
 Element level: k4_testing_rgbnet runs a scene's packed rgbnet on rows the test supplies, with the device code of one MLP
-mode -- mlp_batch_wgmma on a ring tile written through the scene's column map (tc / ws), MmaWarpCtx driven as k4_march.cu
+mode -- mlp_batch_wgmma on a ring tile written through the scene's column map (ws), MmaWarpCtx driven as k4_march.cu
 drives it (f16 / f16x3), mlp_fp32 (fp32) -- and returns what the marchers accumulate into a ray: per group of G rows
 (128 for wgmma, 32 otherwise) and owner j, the sum of w * sigmoid(logit (+ diffuse)) over the rows j owns.  The models are
 the 12 wgmma configurations of csrc/k4_ws_cfgs.h at their exact shapes plus the models of test_gpu_marcher.WS_SHAPES that
 run zero-padded on a larger configuration; every model runs in every mode it has a build for.
 
-Per ray: the ws marcher against the tc marcher, which do the same arithmetic per sample and differ only in the order of
-their shared-memory atomics, on scenes that stress the ring (long queues next to empty rays, one live ray per tile, more
-tiles than marcher groups); and every tensor-core mode against fp32 mode on every WS_SHAPES model, bounded per sample
-with the weights and rgbnet inputs that oracle.pipeline.forward(trace=...) records.  This is what checks the row
+Per ray: every tensor-core mode against fp32 mode on every WS_SHAPES model, and ws against fp32 mode on scenes that
+stress the ring (long queues next to empty rays, one live ray per tile, more tiles than marcher groups), bounded per
+sample with the weights and rgbnet inputs that oracle.pipeline.forward(trace=...) records.  This is what checks the row
 assembly of the marchers themselves (k0 channels, position code, view embedding, the column map of a padded wgmma
 configuration, the diffuse logits) and which ray a sample is credited to.
 
@@ -352,48 +351,106 @@ def test_random_operands_within_bound(cuda_device, spec):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# 3. per ray: ws against tc (the same arithmetic per sample), on scenes that stress the ring
+# 3. per ray: every tensor-core mode against fp32 mode, with the per-sample inputs of the CPU oracle
 # ---------------------------------------------------------------------------------------------------------------------
-def ray_bound(out, n_c, bg):
-    """|a - b| per ray for two renders that add the same terms w sigma in different orders: each sum is within
-    (n_c - 1) u sum w sigma of the exact one, so the two within twice that, plus the final rounding of the background add
-    in each.  sum w sigma is taken from a's colour minus its background, inflated by the rounding of that difference."""
-    T = out['alphainv_last'].double()[:, None]
-    rgb = out['rgb_marched'].double()
-    s = (rgb - T * bg).abs() * (1 + 2 * U) + 2 * U * rgb.abs()
-    return 2 * (n_c.double()[:, None] - 1).clamp(min=0) * U * s + 2 * U * rgb.abs()
+def check_per_ray_against_fp32(m, st, spec, rays, kw, runs, dev, label, act=None):
+    """Renders `runs` ((mode, image_hw) pairs) and fp32 mode (in the first run's order) and bounds every run's colour per
+    ray against fp32's.  The marchers march bit-identically in every mode, so per ray the colours of a tensor-core mode
+    and of fp32 mode differ only through the MLP on the same samples.  The oracle's trace gives each shaded sample's
+    weight and rgbnet inputs; per sample both logits lie within their bounds of the unquantised fp64 model
+    (true_logit_bound, or mpi_act.act_logit_bound for a hidden activation `act`), so
 
+        |rgb_mode - rgb_fp32| <= sum_i w_i [sigma'_max (L_mode,i + L_fp32,i) + 2 * SIG_REL * sigma_hi + 2 u sigma_hi]
+                                 + 2 (n - 1) u sum_i w_i sigma_hi + 2 u |rgb|
 
-def compare_ws_tc(m, ro, rd, vd, kw, hw, label):
-    outs = {}
-    for mode in ('ws', 'tc'):
-        for h in ((hw, None) if hw else (None,)):
-            outs[(mode, h)] = m.render_rays(ro, rd, vd, kw, image_hw=h, mlp_mode=mode, debug=True)
+    (the two sigmoids, the two products w * sigma, the two sums of n terms, the two background adds).  The GPU weight of a
+    sample is taken as the oracle's times 1 + 1e-4, and the GPU inputs within FEAT_REL of the oracle's.  Every run's
+    alphainv_last and ray_stats equal fp32's on every ray.  Rays whose in-box, occupied or shaded sample counts differ
+    from the oracle's (a sample at a threshold) are left out of the bound; at most 1e-3 of the rays may be.
+    Returns (n_c, bad): the oracle's shaded samples per ray and the rays left out."""
+    from oracle import ops, pipeline
+    import contextlib
+    import mpi_act
+    ro, rd, vd = rays
+    stats, trace = {}, {}
+    with mpi_act.oracle_act(act) if act else contextlib.nullcontext():
+        ref = pipeline.forward(st, ro, rd, vd, ops.CpuOps, stats=stats, trace=trace, **kw)
+    args = (ro.to(dev), rd.to(dev), vd.to(dev), kw)
+    fp = m.render_rays(*args, image_hw=runs[0][1], mlp_mode='fp32', debug=True)
+    outs = {(mode, hw): m.render_rays(*args, image_hw=hw, mlp_mode=mode, debug=True) for mode, hw in runs}
     torch.cuda.synchronize()
-    base = outs[('tc', None)]
-    n_c = base['ray_stats'][:, 3].cpu()
-    b = ray_bound({k: v.cpu() for k, v in base.items()}, n_c, float(kw['bg']))
-    worst = 0.0
+    fp = {n: t.cpu() for n, t in fp.items()}
+    N = ro.shape[0]
+    rid = trace['ray_id'].long()
+    n_c = torch.bincount(rid, minlength=N)
+    rs, ors = fp['ray_stats'].long(), ref['_ray_stats']
+    bad = (rs[:, 1] != ors[:, 0]) | (rs[:, 2] != ors[:, 1]) | (rs[:, 3] != n_c)
+    assert int(bad.sum()) <= max(1, int(1e-3 * N)), (label, int(bad.sum()))
+
+    shp = shape_info(types.SimpleNamespace(), spec)
+    shp.layers = [(w_.double().numpy(), b_.double().numpy()) for w_, b_ in st['rgbnet']]
+    x = trace['rgb_feat'].double().numpy()
+    diff = None if trace['diffuse'] is None else trace['diffuse'].double().numpy()
+    w = trace['weights'].double().numpy()[:, None] * (1 + 1e-4)
+    D0 = FEAT_REL * np.abs(x) + 2.0 ** -24
+    if act:
+        bound = lambda mode: mpi_act.act_logit_bound(mode, shp, x, diff, act, D0=D0, true=True)
+    else:
+        bound = lambda mode: true_logit_bound(mode, shp, x, diff, D0)
+    l_f, E_f = bound('fp32')
+    rid_np = rid.numpy()
+    rgb_f = fp['rgb_marched'].double()
+    keep = ~bad.numpy()
+    ratios = {}
     for key, o in outs.items():
-        assert torch.equal(o['alphainv_last'], base['alphainv_last']), (label, key)
-        assert torch.equal(o['ray_stats'], base['ray_stats']), (label, key)
-        d = (o['rgb_marched'].double().cpu() - base['rgb_marched'].double().cpu()).abs()
-        assert (d <= b).all(), (label, key, int((d > b).sum()), float((d / b.clamp(min=1e-300)).max()))
-        worst = max(worst, float((d / b.clamp(min=1e-300)).max()))
-    return n_c, worst
+        o = {n: t.cpu() for n, t in o.items()}
+        assert torch.equal(o['alphainv_last'], fp['alphainv_last']) and torch.equal(o['ray_stats'], fp['ray_stats']), (label, key)
+        l_m, E_m = bound(key[0])
+        assert np.allclose(l_m, l_f, rtol=0, atol=1e-12)
+        Em = np.maximum(E_m, E_f)
+        zc = np.clip(0.0, l_f - Em, l_f + Em)
+        dmax = sig(zc) * (1 - sig(zc))
+        s_hi = sig(l_f + Em)
+        per = w * (dmax * (E_m + E_f) + (2 * SIG_REL + 2 * U) * s_hi)
+        B = np.zeros((N, 3))
+        H = np.zeros((N, 3))
+        np.add.at(B, rid_np, per)
+        np.add.at(H, rid_np, w * s_hi)
+        B += 2 * np.maximum(n_c.numpy()[:, None] - 1, 0) * U * H + 2 * U * rgb_f.abs().numpy()
+        d = (o['rgb_marched'].double() - rgb_f).abs().numpy()
+        ok = d[keep] <= B[keep]
+        assert ok.all(), (label, key, int((~ok).sum()), float((d[keep] / np.maximum(B[keep], 1e-300)).max()))
+        ratios[key] = float((d[keep] / np.maximum(B[keep], 1e-300)).max())
+    print(label, 'per-ray error/bound against fp32', {k: f'{v:.3g}' for k, v in ratios.items()})
+    return n_c, bad
+
+
+def _ray_spec(kind, skw, cid):
+    return ('ray', kind, skw['k0_dim'], skw['viewbase_pe'], skw.get('spatial_pe', 0), skw['width'],
+            int(skw.get('rgbnet_direct', True)), cid)
+
+
+# the rgbnet shapes of make_state's default DirectVoxGO (configs/default.py fine stage) and DirectMPIGO (LLFF) scenes
+WS_RING_SPECS = {'cfgA': _ray_spec('cfgA', dict(k0_dim=12, viewbase_pe=4, width=128), 1),
+                 'cfgB': _ray_spec('cfgB', dict(k0_dim=9, viewbase_pe=0, spatial_pe=0, width=64), 6)}
+
+
+def ws_both_orders(hw):
+    """ws on image tiles (when the rays form an image) and in flat ray order."""
+    return [('ws', hw), ('ws', None)] if hw else [('ws', None)]
 
 
 @pytest.mark.parametrize('kind', ['cfgA', 'cfgB'])
 @pytest.mark.parametrize('regime', ['fog', 'shell', 'blobs'])
-def test_ws_equals_tc_per_ray(cuda_device, kind, regime):
+def test_ws_against_fp32_per_ray(cuda_device, kind, regime):
     if regime == 'blobs':
         st = _blob_state(kind)
     else:
         st = make_state(kind, xy=48, depth=32, regime=regime) if kind == 'cfgB' else make_state(kind, res=48, regime=regime)
     hw = (40, 52)
-    (ro, rd, vd), kw = rays_for(st, *hw)
+    rays, kw = rays_for(st, *hw)
     m = model_from_state(st, cuda_device)
-    n_c, worst = compare_ws_tc(m, ro.to(cuda_device), rd.to(cuda_device), vd.to(cuda_device), kw, hw, (kind, regime))
+    n_c, _ = check_per_ray_against_fp32(m, st, WS_RING_SPECS[kind], rays, kw, ws_both_orders(hw), cuda_device, (kind, regime))
     assert int(n_c.sum()) > 1000
 
 
@@ -410,7 +467,8 @@ def test_ring_long_queues_next_to_empty_rays(cuda_device):
     keep[[3, 77, 140, 141, 255]] = True
     ro = torch.where(keep[:, None], ro, far)
     m = model_from_state(st, cuda_device)
-    n_c, _ = compare_ws_tc(m, ro.to(cuda_device), rd.to(cuda_device), vd.to(cuda_device), kw, None, 'long')
+    n_c, bad = check_per_ray_against_fp32(m, st, WS_RING_SPECS['cfgA'], (ro, rd, vd), kw, ws_both_orders(None), cuda_device, 'long')
+    assert not bad[keep].any()
     assert int(n_c.max()) > 384 and int((n_c == 0).sum()) >= 200, (int(n_c.max()), int((n_c == 0).sum()))
 
 
@@ -423,7 +481,8 @@ def test_ring_one_live_ray_per_tile(cuda_device):
     keep[torch.arange(37, n, 128)] = True
     ro = torch.where(keep[:, None], ro, torch.tensor([0.0, 0.0, 50.0]))
     m = model_from_state(st, cuda_device)
-    n_c, _ = compare_ws_tc(m, ro.to(cuda_device), rd.to(cuda_device), vd.to(cuda_device), kw, None, 'sparse')
+    n_c, bad = check_per_ray_against_fp32(m, st, WS_RING_SPECS['cfgA'], (ro, rd, vd), kw, ws_both_orders(None), cuda_device, 'sparse')
+    assert int(keep.sum()) == 16 and not bad[keep].any()
     assert int((n_c > 0).sum()) == int(keep.sum()) and int(n_c.max()) > 0
 
 
@@ -432,9 +491,9 @@ def test_ring_many_tiles_per_cta(cuda_device):
     56 groups take a second tile and run their FULL / DONE mbarriers on across a tile boundary."""
     st = make_state('cfgA', res=48, regime='shell')
     hw = (128, 320)
-    (ro, rd, vd), kw = rays_for(st, *hw)
+    rays, kw = rays_for(st, *hw)
     m = model_from_state(st, cuda_device)
-    n_c, _ = compare_ws_tc(m, ro.to(cuda_device), rd.to(cuda_device), vd.to(cuda_device), kw, hw, 'many tiles')
+    n_c, _ = check_per_ray_against_fp32(m, st, WS_RING_SPECS['cfgA'], rays, kw, ws_both_orders(hw), cuda_device, 'many tiles')
     assert int(n_c.sum()) > 100000
 
 
@@ -454,34 +513,18 @@ def test_f16x3_without_shared_memory_room_is_unsupported(cuda_device):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# 3b. per ray: every tensor-core mode against fp32 mode, with the per-sample inputs of the CPU oracle
+# 3b. per ray: every tensor-core mode against fp32 mode on every WS_SHAPES model
 # ---------------------------------------------------------------------------------------------------------------------
-RAY_SHAPES = [('cfgA', dict(k0_dim=12, viewbase_pe=4, width=128), 1),       # configs/default.py fine stage (tc, ws)
+RAY_SHAPES = [('cfgA', dict(k0_dim=12, viewbase_pe=4, width=128), 1),       # configs/default.py fine stage
               ('cfgB', dict(k0_dim=9, viewbase_pe=0, spatial_pe=0, width=64), 6)] + WS_SHAPES
-
-
-def _ray_spec(kind, skw, cid):
-    return ('ray', kind, skw['k0_dim'], skw['viewbase_pe'], skw.get('spatial_pe', 0), skw['width'],
-            int(skw.get('rgbnet_direct', True)), cid)
 
 
 @pytest.mark.parametrize('kind,skw,cfg_id', RAY_SHAPES,
                          ids=[f'{k}-{"-".join(f"{a}{b}" for a, b in v.items())}' for k, v, _ in RAY_SHAPES])
-def test_every_mode_against_fp32_per_ray(cuda_device, kind, skw, cfg_id):
-    """The marchers march bit-identically in every mode, so per ray the colours of a tensor-core mode and of fp32 mode
-    differ only through the MLP on the same samples.  The oracle's trace gives each shaded sample's weight and rgbnet
-    inputs; per sample both logits lie within their bounds of the unquantised fp64 model (true_logit_bound), so
-
-        |rgb_mode - rgb_fp32| <= sum_i w_i [sigma'_max (L_mode,i + L_fp32,i) + 2 * SIG_REL * sigma_hi + 2 u sigma_hi]
-                                 + 2 (n - 1) u sum_i w_i sigma_hi + 2 u |rgb|
-
-    (the two sigmoids, the two products w * sigma, the two sums of n terms, the two background adds).  The GPU weight of a
-    sample is taken as the oracle's times 1 + 1e-4, and the GPU inputs within FEAT_REL of the oracle's.  Rays whose
-    in-box, occupied or shaded sample counts differ from the oracle's (a sample at a threshold) are excluded; at most
-    1e-3 of the rays may be."""
-    from oracle import ops, pipeline
+def test_tensor_core_modes_against_fp32_per_ray(cuda_device, kind, skw, cfg_id):
+    """check_per_ray_against_fp32 for every tensor-core mode the shape has a build for, on image tiles; the others
+    report an unsupported configuration."""
     from k4nerf import _lib
-    from helpers import model_from_state as mfs
     dev = cuda_device
     if kind == 'cfgB':
         st = make_state(kind, xy=40, depth=24, regime='fog', **skw)
@@ -489,60 +532,15 @@ def test_every_mode_against_fp32_per_ray(cuda_device, kind, skw, cfg_id):
     else:
         st = make_state(kind, res=40, regime='fog', **skw)
         hw = (32, 40)
-    (ro, rd, vd), kw = rays_for(st, *hw, **({'radius': 0.6} if kind == 'cfgC' else {}))
-    stats, trace = {}, {}
-    ref = pipeline.forward(st, ro, rd, vd, ops.CpuOps, stats=stats, trace=trace, **kw)
-    m = mfs(st, dev)
+    rays, kw = rays_for(st, *hw, **({'radius': 0.6} if kind == 'cfgC' else {}))
+    m = model_from_state(st, dev)
     spec = _ray_spec(kind, skw, cfg_id)
-    outs = {}
-    for mode in ('fp32', 'f16', 'f16x3', 'tc', 'ws'):
-        if mode == 'tc' and kind == 'cfgC':
-            continue                     # DirectContractedVoxGO runs 'tc' on the ws kernel (k4nerf/dcvgo.py)
+    runs = []
+    for mode in ('f16', 'f16x3', 'ws'):
         if supports(spec, mode):
-            outs[mode] = m.render_rays(ro.to(dev), rd.to(dev), vd.to(dev), kw, image_hw=hw, mlp_mode=mode, debug=True)
+            runs.append((mode, hw))
         else:
             with pytest.raises(_lib.K4Error, match='unsupported configuration'):
-                m.render_rays(ro.to(dev), rd.to(dev), vd.to(dev), kw, image_hw=hw, mlp_mode=mode)
-    torch.cuda.synchronize()
-    outs = {k: {n: t.cpu() for n, t in o.items()} for k, o in outs.items()}
-    fp = outs['fp32']
-    N = ro.shape[0]
-    rid = trace['ray_id'].long()
-    n_c = torch.bincount(rid, minlength=N)
-    rs, ors = fp['ray_stats'].long(), ref['_ray_stats']
-    bad = (rs[:, 1] != ors[:, 0]) | (rs[:, 2] != ors[:, 1]) | (rs[:, 3] != n_c)
-    assert int(bad.sum()) <= max(1, int(1e-3 * N)), int(bad.sum())
+                m.render_rays(*[t.to(dev) for t in rays], kw, image_hw=hw, mlp_mode=mode)
+    n_c, _ = check_per_ray_against_fp32(m, st, spec, rays, kw, runs, dev, (kind, skw))
     assert int(n_c.sum()) > 1000
-
-    shp = shape_info(types.SimpleNamespace(), spec)
-    shp.layers = [(w_.double().numpy(), b_.double().numpy()) for w_, b_ in st['rgbnet']]
-    x = trace['rgb_feat'].double().numpy()
-    diff = None if trace['diffuse'] is None else trace['diffuse'].double().numpy()
-    w = trace['weights'].double().numpy()[:, None] * (1 + 1e-4)
-    D0 = FEAT_REL * np.abs(x) + 2.0 ** -24
-    l_f, E_f = true_logit_bound('fp32', shp, x, diff, D0)
-    rid_np = rid.numpy()
-    rgb_f = fp['rgb_marched'].double()
-    ratios = {}
-    for mode, o in outs.items():
-        if mode == 'fp32':
-            continue
-        assert torch.equal(o['alphainv_last'], fp['alphainv_last']) and torch.equal(o['ray_stats'], fp['ray_stats']), mode
-        l_m, E_m = true_logit_bound(mode, shp, x, diff, D0)
-        assert np.allclose(l_m, l_f, rtol=0, atol=1e-12)
-        Em = np.maximum(E_m, E_f)
-        zc = np.clip(0.0, l_f - Em, l_f + Em)
-        dmax = sig(zc) * (1 - sig(zc))
-        s_hi = sig(l_f + Em)
-        per = w * (dmax * (E_m + E_f) + (2 * SIG_REL + 2 * U) * s_hi)
-        B = np.zeros((N, 3))
-        H = np.zeros((N, 3))
-        np.add.at(B, rid_np, per)
-        np.add.at(H, rid_np, w * s_hi)
-        B += 2 * np.maximum(n_c.numpy()[:, None] - 1, 0) * U * H + 2 * U * rgb_f.abs().numpy()
-        d = (o['rgb_marched'].double() - rgb_f).abs().numpy()
-        keep = ~bad.numpy()
-        ok = d[keep] <= B[keep]
-        assert ok.all(), (mode, int((~ok).sum()), float((d[keep] / np.maximum(B[keep], 1e-300)).max()))
-        ratios[mode] = float((d[keep] / np.maximum(B[keep], 1e-300)).max())
-    print(kind, skw, 'per-ray error/bound against fp32', {k: f'{v:.3g}' for k, v in ratios.items()})

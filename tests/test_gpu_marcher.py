@@ -16,7 +16,7 @@ from helpers import compare, make_state, model_from_state, rays_for
 
 pytestmark = pytest.mark.gpu
 
-PSNR_BAR = {'fp32': 80.0, 'f16x3': 70.0, 'f16': 70.0, 'tc': 70.0, 'ws': 70.0}
+PSNR_BAR = {'fp32': 80.0, 'f16x3': 70.0, 'f16': 70.0, 'ws': 70.0}
 
 
 def run_both(st, rays, kw, dev, mode, image_hw=None):
@@ -51,7 +51,7 @@ def check_geometry(ours, ref, stats, st, n):
 
 
 @pytest.mark.parametrize('regime', ['fog', 'shell'])
-@pytest.mark.parametrize('mode', ['fp32', 'f16x3', 'f16', 'tc', 'ws'])
+@pytest.mark.parametrize('mode', ['fp32', 'f16x3', 'f16', 'ws'])
 def test_cfgA_parity(cuda_device, regime, mode):
     st = make_state('cfgA', res=48, regime=regime)
     rays, kw = rays_for(st, 40, 52)
@@ -64,7 +64,7 @@ def test_cfgA_parity(cuda_device, regime, mode):
     assert cmp['depth_maxabs'] <= 2e-5, cmp
 
 
-@pytest.mark.parametrize('mode', ['fp32', 'f16x3', 'tc', 'ws'])
+@pytest.mark.parametrize('mode', ['fp32', 'f16x3', 'ws'])
 def test_cfgA_2d_tiles_equal_linear_order(cuda_device, mode):
     """8x4 pixel-tile scheduling must not change any ray's result."""
     st = make_state('cfgA', res=32, regime='shell')
@@ -79,7 +79,7 @@ def test_cfgA_2d_tiles_equal_linear_order(cuda_device, mode):
     if mode == 'fp32':
         assert torch.equal(a['rgb_marched'], b['rgb_marched'])
     else:
-        assert (a['rgb_marched'] - b['rgb_marched']).abs().max().item() < (1e-5 if mode not in ('tc', 'ws') else 2e-5)
+        assert (a['rgb_marched'] - b['rgb_marched']).abs().max().item() < (1e-5 if mode != 'ws' else 2e-5)
 
 
 def test_cfgA_not_direct_and_width64(cuda_device):
@@ -104,7 +104,7 @@ def test_cfg1_colour_grid_no_mlp(cuda_device):
 
 
 @pytest.mark.parametrize('regime', ['fog', 'shell'])
-@pytest.mark.parametrize('mode', ['fp32', 'f16x3', 'f16', 'tc', 'ws'])
+@pytest.mark.parametrize('mode', ['fp32', 'f16x3', 'f16', 'ws'])
 def test_cfgB_mpi_parity(cuda_device, regime, mode):
     st = make_state('cfgB', xy=48, depth=32, regime=regime)
     rays, kw = rays_for(st, 30, 40)
@@ -142,11 +142,11 @@ def test_edge_cases(cuda_device):
     ro, rd, vd = ro.repeat(9, 1)[:33], rd.repeat(9, 1)[:33], vd.repeat(9, 1)[:33]
     stats = {}
     ref = pipeline.forward(st, ro, rd, vd, ops.CpuOps, stats=stats, **kw)
-    for mode in ('fp32', 'f16x3', 'tc', 'ws'):
+    for mode in ('fp32', 'f16x3', 'ws'):
         ours = m.render_rays(ro.to(dev), rd.to(dev), vd.to(dev), kw, mlp_mode=mode, debug=True)
         check_geometry(ours, ref, stats, st, 33)
         cmp = compare(ours, ref, 33)
-        assert cmp['rgb_marched_maxabs'] < (1e-4 if mode not in ('tc', 'ws') else 5e-3), (mode, cmp)
+        assert cmp['rgb_marched_maxabs'] < (1e-4 if mode != 'ws' else 5e-3), (mode, cmp)
         assert torch.equal(ours['alphainv_last'][1].cpu(), torch.tensor(1.0))   # missed the box: T stays 1
 
 
@@ -303,7 +303,7 @@ def test_empty_space_skipping_preserves_results(cuda_device, kind, regime, monke
     check_geometry(outs[(True, 'ws', (96, 128))], ref, stats, st, ro.shape[0])
 
 
-@pytest.mark.parametrize('mode', ['f16x3', 'ws', 'tc', 'fp32'])
+@pytest.mark.parametrize('mode', ['f16x3', 'ws', 'fp32'])
 def test_render_rays_frames_assembles_the_block_cyclic_frame(cuda_device, mode):
     """k4_render_rays_frames: every rank's rows (8-row blocks dealt round-robin) stored by the kernel straight into the
     image-order frames -- here three 'ranks' one after the other on one GPU, two destination frames each (on a multi-GPU

@@ -3,8 +3,8 @@
 1. Per sample (k4_testing_rgbnet): every mode each MPI shape has, on ws configs 6, 7, 8 and on a model padded into
    config 6 (width 48, 7 k0 channels: its padded hidden units have gauss(0) = 1 and must meet zero outgoing weights),
    against the fp64 model within the error model of mpi_act.act_logit_bound.
-2. Per ray: every mode against fp32 mode (as test_gpu_march_mlp.test_every_mode_against_fp32_per_ray), ws against tc,
-   and the geometry (S_m, S_d, alphainv_last) bit-identical to the relu model of the same grids.
+2. Per ray: every mode against fp32 mode (as test_gpu_march_mlp.check_per_ray_against_fp32), ws also on scenes of its
+   own in both ray orders, and the geometry (S_m, S_d, alphainv_last) bit-identical to the relu model of the same grids.
 3. At scale: the [384,384,256] LLFF model at 1008x756 against the reference's kernels + ATen (oracle on RefExtOps).
 4. End to end: a gauss checkpoint through utils.load_model and render_viewpoints with NDC rays; forward under autograd.
 Every scene's rgbnet is scaled so that the activation is exercised (mpi_act.scale_for_act / assert_exercised).
@@ -25,17 +25,11 @@ from mpi_act import ACTS, act_logit_bound, assert_exercised, mpi_model, oracle_a
 
 pytestmark = pytest.mark.gpu
 
-MODES = {'fp32': 0, 'f16': 1, 'f16x3': 2, 'tc': 3, 'ws': 4}
+MODES = {'fp32': 0, 'f16': 1, 'f16x3': 2, 'ws': 4}
 ROWS = [1, 33, 64, 128, 300]
 # (name, kind, C, vpe, spe, width, direct, config id)
 SHAPES = [('cfg6', 'cfgB', 9, 0, 0, 64, 1, 6), ('cfg7', 'cfgB', 12, 4, 0, 128, 1, 7), ('cfg8', 'cfgB', 12, 4, 5, 128, 1, 8),
           ('C7-w48-on6', 'cfgB', 7, 0, 0, 48, 1, 6)]
-
-
-def _supports(spec, mode):
-    if mode == 'tc':                                    # k4_march_tc.cu: CfgB only among the MPI shapes
-        return spec[1:7] == ('cfgB', 9, 0, 0, 64, 1)
-    return supports(spec, mode)
 
 
 class ActModel:
@@ -121,11 +115,11 @@ def test_every_mode_per_sample_within_bound(cuda_device, spec, act):
     w = np.maximum(rng.random(300), 1e-3).astype(np.float32).astype(np.float64)
     ratios = {}
     for mode in MODES:
-        if not _supports(spec, mode):
+        if not supports(spec, mode):
             continue
         for n in ROWS:
             xs, ws = x[:n], w[:n]
-            G = 128 if mode in ('ws', 'tc') else 32
+            G = 128 if mode == 'ws' else 32
             for owner in (np.concatenate([rng.permutation(G)[:min(G, n - s)] for s in range(0, n, G)]).astype(np.int32),
                           rng.integers(0, 3, size=n).astype(np.int32)):
                 racc, Gk = m.run(mode, xs, ws, owner)
@@ -149,7 +143,7 @@ RAY_SHAPES = [(dict(k0_dim=9, viewbase_pe=0, spatial_pe=0, width=64), 6), (dict(
 @pytest.mark.parametrize('act', ACTS)
 @pytest.mark.parametrize('skw,cfg_id', RAY_SHAPES, ids=['llff', 'cfg8'])
 def test_every_mode_against_fp32_per_ray(cuda_device, skw, cfg_id, act):
-    """The bound of test_gpu_march_mlp.test_every_mode_against_fp32_per_ray with the activation's error model, and the
+    """The bound of test_gpu_march_mlp.check_per_ray_against_fp32 with the activation's error model, and the
     geometry of every mode bit-identical to the relu model of the same grids."""
     from oracle import ops, pipeline
     dev = cuda_device
@@ -166,7 +160,7 @@ def test_every_mode_against_fp32_per_ray(cuda_device, skw, cfg_id, act):
     outs, routs = {}, {}
     args = (ro.to(dev), rd.to(dev), vd.to(dev), kw)
     for mode in MODES:
-        if _supports(spec, mode):
+        if supports(spec, mode):
             outs[mode] = m.render_rays(*args, image_hw=hw, mlp_mode=mode, debug=True)
             routs[mode] = relu.render_rays(*args, image_hw=hw, mlp_mode=mode, debug=True)
     torch.cuda.synchronize()
@@ -213,17 +207,18 @@ def test_every_mode_against_fp32_per_ray(cuda_device, skw, cfg_id, act):
 
 @pytest.mark.parametrize('act', ACTS)
 @pytest.mark.parametrize('regime', ['fog', 'shell'])
-def test_ws_equals_tc_per_ray(cuda_device, act, regime):
-    """CfgB (the LLFF shape): the ws and tc kernels run the same arithmetic per sample; per ray they differ only in the
-    order of the colour sums (test_gpu_march_mlp.compare_ws_tc)."""
-    from test_gpu_march_mlp import compare_ws_tc
+def test_ws_against_fp32_per_ray(cuda_device, act, regime):
+    """The LLFF shape (configuration 6): ws on image tiles and in flat ray order within the per-ray bound of
+    test_gpu_march_mlp.check_per_ray_against_fp32 against fp32 mode, with the activation's error model."""
+    from test_gpu_march_mlp import WS_RING_SPECS, check_per_ray_against_fp32, ws_both_orders
     st = make_state('cfgB', xy=48, depth=32, regime=regime)
     x = scale_state_rgbnet(st, act)
     assert_exercised([(W.double().numpy(), b.double().numpy()) for W, b in st['rgbnet']], x, act)
     hw = (40, 52)
-    (ro, rd, vd), kw = rays_for(st, *hw)
+    rays, kw = rays_for(st, *hw)
     m = mpi_model(st, act, cuda_device)
-    n_c, _ = compare_ws_tc(m, ro.to(cuda_device), rd.to(cuda_device), vd.to(cuda_device), kw, hw, (act, regime))
+    n_c, _ = check_per_ray_against_fp32(m, st, WS_RING_SPECS['cfgB'], rays, kw, ws_both_orders(hw), cuda_device, (act, regime),
+                                        act=act)
     assert int(n_c.sum()) > 1000
 
 

@@ -131,10 +131,10 @@ def test_cfgC_contracted_160(ref_ops, cuda_device):
 
 
 @pytest.mark.parametrize('regime', ['fog', 'shell'])
-@pytest.mark.parametrize('mode', ['tc', 'ws'])
+@pytest.mark.parametrize('mode', ['ws'])
 def test_persistent_multi_tile_vs_gpu_oracle(ref_ops, cuda_device, regime, mode):
     """More 128-ray tiles than warpgroups on the chip at a small grid (both warpgroups of every CTA busy,
-    several tiles each, ragged batches): both wgmma kernels against the reference kernels' pipeline,
+    several tiles each, ragged batches): the wgmma kernel against the reference kernels' pipeline,
     in 2-D tile order and in linear order."""
     dev = cuda_device
     st = make_state('cfgA', res=48, regime=regime)

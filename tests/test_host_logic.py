@@ -119,7 +119,12 @@ def test_dcvgo_constructor_contract():
     n_inner = int(2 / (2 + 2 * 0.2) * m.world_len / 0.5) + 1
     assert t.numel() == 2 * n_inner and bool((t[1:] > t[:-1]).all())
     assert abs(float(t[0]) - 1.0 / n_inner) < 1e-6 and float(t[-1]) > 100
-    assert m.resolve_mlp_mode('tc') == 'ws' and m.resolve_mlp_mode('fp32') == 'fp32'
+    dvgo = k4nerf.DirectVoxGO([-1] * 3, [1] * 3, num_voxels=8 ** 3, num_voxels_base=8 ** 3, alpha_init=1e-2,
+                              fast_color_thres=1e-4, rgbnet_dim=12)
+    dmpigo = k4nerf.DirectMPIGO([-1] * 3, [1] * 3, num_voxels=8 ** 3, mpi_depth=8, fast_color_thres=1e-3, rgbnet_dim=9,
+                                rgbnet_width=64, act_type='relu', mode_type='mlp')
+    for km in (m, dvgo, dmpigo):                      # 'tc' / 'tcgen05' (K4_MLP_TCGEN05) alias the wgmma marcher 'ws'
+        assert km.resolve_mlp_mode('tc') == km.resolve_mlp_mode('tcgen05') == 'ws' and km.resolve_mlp_mode('fp32') == 'fp32'
     with pytest.raises(RuntimeError):                 # 'auto' asks the library which kernels cover the DEVICE scene: no CPU path
         m.resolve_mlp_mode('auto')
     with pytest.raises(NotImplementedError):

@@ -57,8 +57,9 @@ def test_compositions_hit_their_targets(cfg, order):
     assert per_step[0] == 50 and (per_step[1:-1] == 128).all() and per_step[-1] == 78 and len(per_step) > 20
     pend = np.cumsum(per_step)[:-1] % 128
     assert ((per_step[1:] == 128) & (pend == 50)).sum() == len(per_step) - 2
-    assert rep['ws'] == rep['tc'] + sum(1 for x in ws if x[2]) and rep['ws_lo'] == rep['tc']
-    assert rep['ws_hi'] == rep['tc'] + sum(1 for x in ws if x[1] % 128 == 0 and x[1] > 0)
+    assert rep['ws_lo'] == sum(-(-int(n) // 128) for n in n_t)
+    assert rep['ws'] == rep['ws_lo'] + sum(1 for x in ws if x[2])
+    assert rep['ws_hi'] == rep['ws_lo'] + sum(1 for x in ws if x[1] % 128 == 0 and x[1] > 0)
 
 
 @pytest.mark.parametrize('cfg', sorted(mb.CFGS))

@@ -16,7 +16,7 @@ from helpers import compare, make_state, model_from_state, rays_for  # noqa: E40
 
 def main():
     dev = torch.device('cuda', 0)
-    modes = sys.argv[1:] or ['fp32', 'f16x3', 'f16', 'tc', 'ws']
+    modes = sys.argv[1:] or ['fp32', 'f16x3', 'f16', 'ws']
     cases = [('cfgA', dict(res=96, regime='fog'), (96, 128)), ('cfgA', dict(res=96, regime='shell'), (96, 128)),
              ('cfgB', dict(xy=96, depth=64, regime='fog'), (72, 96)), ('cfgB', dict(xy=96, depth=64, regime='shell'), (72, 96))]
     have_ref = os.path.exists(ops.ref_ext_path())

@@ -19,7 +19,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--res', type=int, default=160)
     ap.add_argument('--hw', type=int, nargs=2, default=[756, 1008])
-    ap.add_argument('--modes', nargs='+', default=['ws', 'tc'])
+    ap.add_argument('--modes', nargs='+', default=['ws'])
     ap.add_argument('--regimes', nargs='+', default=['fog', 'shell'])
     ap.add_argument('--kind', default='cfgA')
     ap.add_argument('--iters', type=int, default=5)
