@@ -12,6 +12,7 @@ K4_ACT_RELU, K4_ACT_GAUSS, K4_ACT_LKRELU = 0, 1, 2
 K4_MAX_MLP_LAYERS = 8
 K4_MAX_PEERS = 8
 K4_MASKED_QUANTILES_HIST_LEN = 4 * 2048 + 2
+K4_PNG_SEG = 32768
 MLP_MODES = {'fp32': K4_MLP_FP32, 'f16': K4_MLP_F16, 'f16x3': K4_MLP_F16X3, 'ws': K4_MLP_TCGEN05_WS}
 
 
@@ -242,6 +243,10 @@ EXPORTS = {
                                        C.c_void_p, C.c_void_p]),
     'k4_op_frame_u8': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.POINTER(C.c_int64), C.c_int32, C.c_int32, C.c_void_p,
                                  C.c_void_p]),
+    'k4_png_encode_bound': (C.c_size_t, [C.c_int64, C.c_int64]),
+    'k4_png_workspace_bytes': (C.c_size_t, [C.c_int64, C.c_int64]),
+    'k4_png_encode': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t,
+                                C.c_void_p]),
     'k4_make_rays_rows':(C.c_int, [C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_int32,
                                     C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'k4_make_rays': (C.c_int, [C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_int32,

@@ -184,6 +184,12 @@ def render_frame_4k(model, net_sr, H, W, K, c2w, ndc, render_kwargs, test_tile=5
 
     Returns ``(sr [3,s*H,s*W] float32 in [0,1] or uint8 [s*H,s*W,3], lr dict)`` -- same values as
     ``render_viewpoints_sr`` followed by ``SFTNet.tile_process`` and ``clamp(0,1)``."""
+    sr, lr, _ = _render_frame_4k(model, net_sr, H, W, K, c2w, ndc, render_kwargs, test_tile, out_u8, flip_x, flip_y)
+    return sr, lr
+
+
+def _render_frame_4k(model, net_sr, H, W, K, c2w, ndc, render_kwargs, test_tile, out_u8, flip_x, flip_y):
+    """:func:`render_frame_4k` and the frame's ``viewdirs`` ``[H*W, 3]``."""
     from .sr_esrnet import sft_condition
     rays_o, rays_d, viewdirs = dvgo.get_rays_of_a_view(
         H, W, K, torch.as_tensor(np.asarray(c2w), dtype=torch.float32), ndc,
@@ -197,7 +203,50 @@ def render_frame_4k(model, net_sr, H, W, K, c2w, ndc, render_kwargs, test_tile=5
     sr = sr.squeeze(0).clamp_(0, 1)
     if out_u8:
         sr = (sr * 255).to(torch.uint8).permute(1, 2, 0).contiguous()     # to8b: (255*clip(x,0,1)).astype(uint8)
-    return sr, lr
+    return sr, lr, viewdirs.view(-1, 3)
+
+
+@torch.no_grad()
+def render_test_4k(model, net_sr, render_poses, HW, Ks, ndc, render_kwargs, gt_imgs=None, savedir=None, ckpt_name='',
+                   dump_images=False, eval_ssim=False, eval_lpips_alex=False, eval_lpips_vgg=False, global_step=0,
+                   test_tile=510, flip_x=None, flip_y=None):
+    """run_sr.py --render_test (run_sr.py:1340-1396) with every frame rendered and written from the device.
+
+    Each view is one :func:`render_frame_4k` pass (march, decode, quantise), with no numpy round trip between the
+    marcher and the decoder.  The LR results are what :func:`render_viewpoints_sr` returns on the same inputs, bit for
+    bit: ``(rgbs, depths, bgmaps, psnrs, viewdirs_all, rgb_features)``; with ``gt_imgs`` the PSNR is computed and
+    SSIM / LPIPS scored and printed as there.  With ``savedir``: ``dump_images`` writes the LR frames as
+    ``e<global_step>_<i>.png`` (the pixels of ``render_viewpoints_sr``'s dumps), and every SR frame is written as
+    ``<ckpt_name>_<i>.png``, ``to8b`` of the clamped decoder output; both are encoded on the GPU
+    (:func:`k4nerf.utils.png_encode`).  ``ckpt_name`` is the reference's ``ckpt_path.split('/')[-1][:-4]``."""
+    import os
+    from .utils import frame_u8_cuda, write_png
+    assert len(render_poses) == len(HW) and len(HW) == len(Ks)
+    flip_x = render_kwargs.get('flip_x', False) if flip_x is None else flip_x
+    flip_y = render_kwargs.get('flip_y', False) if flip_y is None else flip_y
+    rgbs, rgb_features, depths, bgmaps, psnrs, ssims, viewdirs_all = [], [], [], [], [], [], []
+    lpips_alex, lpips_vgg = [], []
+    for i, c2w in enumerate(render_poses):
+        H, W = int(HW[i][0]), int(HW[i][1])
+        sr, lr, viewdirs = _render_frame_4k(model, net_sr, H, W, Ks[i], c2w, ndc, render_kwargs, test_tile, True,
+                                            flip_x, flip_y)
+        rgb_f = lr['rgb_marched'].view(H, W, 3)
+        rgb_d = rgb_f.clamp(0, 1)
+        rgb = rgb_d.cpu().numpy()
+        rgbs.append(rgb)
+        rgb_features.append(rgb_f.cpu().numpy())
+        depths.append(lr['depth'].view(H, W, 1).cpu().numpy())
+        bgmaps.append(lr['alphainv_last'].view(H, W, 1).cpu().numpy())
+        viewdirs_all.append(viewdirs)
+        if gt_imgs is not None:
+            psnrs.append(-10. * np.log10(np.mean(np.square(rgb - gt_imgs[i]))))
+            _score(rgb_d, gt_imgs[i], eval_ssim, eval_lpips_alex, eval_lpips_vgg, ssims, lpips_alex, lpips_vgg)
+        if savedir is not None:
+            if dump_images:
+                write_png(os.path.join(savedir, 'e{}_{:03d}.png'.format(global_step, i)), frame_u8_cuda(rgb_f))
+            write_png(os.path.join(savedir, '{}_{:03d}.png'.format(ckpt_name, i)), sr)
+    _report(psnrs, ssims, lpips_vgg, lpips_alex)
+    return np.array(rgbs), np.array(depths), np.array(bgmaps), psnrs, viewdirs_all, np.array(rgb_features)
 
 
 @torch.no_grad()

@@ -550,3 +550,46 @@ def frame_u8_cuda(rgb, render_video_flipy=False, render_video_rot90=0, out=None)
         _cuda_call('k4_op_frame_u8', C.c_void_p(rgb.data_ptr()), H, W, _strides3(rgb), int(bool(render_video_flipy)), k,
                    C.c_void_p(out.data_ptr()), C.c_void_p(torch.cuda.current_stream(rgb.device).cuda_stream))
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# PNG files of uint8 frames (run.py:165, run_sr.py:175 / 1396: imageio.imwrite)
+# ------------------------------------------------------------------------------------------------
+def png_encode(frame):
+    """The PNG file of a contiguous uint8 ``[H, W, 3]`` CUDA frame, encoded on its device by ``k4_png_encode``
+    (csrc/k4_png.cu), as ``bytes``.  The encode is queued on the current stream; the only host synchronisations are
+    the copy of the file's length and then of its bytes."""
+    import ctypes as C
+    from . import _lib
+    if not (_is_cuda(frame) and frame.dtype == torch.uint8 and frame.ndim == 3 and frame.shape[-1] == 3):
+        raise ValueError(f'png_encode: a uint8 [H, W, 3] CUDA tensor expected, got {getattr(frame, "dtype", type(frame))} '
+                         f'{tuple(getattr(frame, "shape", ()))}')
+    frame = frame.detach().contiguous()
+    H, W = frame.shape[0], frame.shape[1]
+    dev = frame.device
+    bound = _lib.lib.k4_png_encode_bound(H, W)
+    if bound == 0:
+        raise ValueError(f'png_encode: a {H} x {W} frame does not fit one PNG IDAT chunk')
+    with torch.cuda.device(dev):
+        ws = torch.empty(_lib.lib.k4_png_workspace_bytes(H, W), dtype=torch.uint8, device=dev)
+        out = torch.empty(bound, dtype=torch.uint8, device=dev)
+        n = torch.empty((), dtype=torch.int64, device=dev)
+        _cuda_call('k4_png_encode', C.c_void_p(frame.data_ptr()), H, W, C.c_void_p(out.data_ptr()), bound,
+                   C.c_void_p(n.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(),
+                   C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+        return out[:int(n.item())].cpu().numpy().tobytes()
+
+
+def write_png(filename, frame):
+    """Write ``frame`` as the PNG file ``filename``: a uint8 ``[H, W, 3]`` CUDA tensor is encoded on its device
+    (:func:`png_encode`), a numpy array goes through the host writer ``render_viewpoints``' dumps use
+    (``render._write_png``: imageio, PIL or cv2).  Anything else raises ``TypeError``."""
+    if _is_cuda(frame):
+        data = png_encode(frame)
+        with open(filename, 'wb') as f:
+            f.write(data)
+    elif isinstance(frame, np.ndarray):
+        from .render import _write_png
+        _write_png(filename, frame)
+    else:
+        raise TypeError(f'write_png: a CUDA tensor or a numpy array expected, got {type(frame).__name__}')

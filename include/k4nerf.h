@@ -888,6 +888,28 @@ K4_API int k4_testing_lpips_stage(const k4_lpips* net, const float* d_img, const
                                   int32_t stage, void* d_out, int64_t out_shape[3], void* d_workspace, size_t workspace_bytes,
                                   k4_stream_t stream);
 
+/*
+ * PNG files of uint8 RGB frames on the device, for run_sr.py --render_test's imageio.imwrite of every frame
+ * (csrc/k4_png.cu; DESIGN.md section 3.10).
+ *   d_rgb: u8 [H, W, 3] contiguous (frame_u8 / render_frame_4k(out_u8=True)'s layout).
+ *   d_out: receives the whole file (signature, IHDR, one IDAT, IEND); out_capacity >= k4_png_encode_bound(H, W).
+ *   d_len: one device int64 (8-byte aligned), receives the file's length in bytes.
+ *   d_workspace: k4_png_workspace_bytes(H, W) bytes, 256-byte aligned.
+ * Each row is filtered with the least sum of |byte as int8| of the five PNG filters (ties to the lowest type); the
+ * filtered stream is cut into segments of K4_PNG_SEG bytes, each one dynamic-Huffman block (code lengths <= 15) with
+ * back-references up to 32 KiB before its start, or one stored block when that is not larger; a dynamic segment
+ * other than the last ends with an empty stored block (a sync flush).  The output is a fixed function of the frame.
+ * The bound is the all-stored file: H (1 + 3 W) + 5 ceil(H (1 + 3 W) / K4_PNG_SEG) + 63 bytes.  Frames whose bound
+ * exceeds 2^31 - 1 (one IDAT chunk) give 0 from both size functions.
+ * A NULL pointer, H or W < 1, too large a frame, out_capacity below the bound, too small or misaligned a workspace:
+ * K4_ERR_INVALID_ARG before any CUDA call.  Caller's stream, no host sync, no allocation.
+ */
+#define K4_PNG_SEG 32768
+K4_API size_t k4_png_encode_bound(int64_t H, int64_t W);
+K4_API size_t k4_png_workspace_bytes(int64_t H, int64_t W);
+K4_API int k4_png_encode(const uint8_t* d_rgb, int64_t H, int64_t W, uint8_t* d_out, size_t out_capacity, int64_t* d_len,
+                         void* d_workspace, size_t workspace_bytes, k4_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
