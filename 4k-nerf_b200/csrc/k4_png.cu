@@ -655,6 +655,31 @@ int launch_error(const char* where) {
     return K4_OK;
 }
 
+// k4_testing_png_code_lengths: huff_lengths on a caller's histogram, one CTA of NT threads as in png_encode_kernel.
+// Histograms package-merge cannot code (more non-zero counts than 2^maxbits, or a total that overflows its 32-bit item
+// weights) get 0xff for every length instead.
+__global__ void __launch_bounds__(NT) png_code_lengths_kernel(const int32_t* __restrict__ freq, int n, int maxbits,
+                                                             uint8_t* __restrict__ len) {
+    __shared__ HuffSmem s;
+    __shared__ int ok;
+    for (int i = threadIdx.x; i < n; i += NT) s.ll_f[i] = freq[i];
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int m = 0;
+        int64_t tot = 0;
+        for (int i = 0; i < n; ++i)
+            if (s.ll_f[i] > 0) { ++m; tot += s.ll_f[i]; }
+        ok = m <= (1 << maxbits) && tot < 0x7fffffff;
+    }
+    __syncthreads();
+    if (!ok) {
+        for (int i = threadIdx.x; i < n; i += NT) len[i] = 0xff;
+        return;
+    }
+    huff_lengths(s.ll_f, n, maxbits, s.ll_l, s);
+    for (int i = threadIdx.x; i < n; i += NT) len[i] = s.ll_l[i];
+}
+
 constexpr size_t MATCH_SMEM = (size_t)(1 << HBITS) * 4 + (WIN + SEG + 16);
 constexpr size_t ENC_SMEM = (size_t)(SEG + OUT_WORDS + 2 + SEG / 32 + 32) * 4;
 
@@ -722,6 +747,12 @@ int k4_png_encode(const uint8_t* d_rgb, int64_t H, int64_t W, uint8_t* d_out, si
     png_crc_kernel<<<(unsigned)((npieces + 255) / 256), 256, 0, st>>>(d_out, misc, npieces, crc);
     png_crc_join_kernel<<<1, NT, 0, st>>>(crc, misc, d_out);
     return launch_error("k4_png_encode launch");
+}
+
+int k4_testing_png_code_lengths(const int32_t* d_freq, int32_t n, int32_t maxbits, uint8_t* d_len, k4_stream_t stream) {
+    if (!d_freq || !d_len || n < 1 || n > MAXSYM || maxbits < 1 || maxbits > 15) return K4_ERR_INVALID_ARG;
+    png_code_lengths_kernel<<<1, NT, 0, (cudaStream_t)stream>>>(d_freq, n, maxbits, d_len);
+    return launch_error("k4_testing_png_code_lengths launch");
 }
 
 }  // extern "C"

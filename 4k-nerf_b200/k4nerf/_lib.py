@@ -263,6 +263,7 @@ EXPORTS = {
                                           C.POINTER(RenderOut), C.c_void_p, C.c_size_t, C.c_void_p, C.c_int32,
                                           C.POINTER(C.c_int32), C.c_void_p]),
     'k4_testing_skip_field': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int32)]),
+    'k4_testing_png_code_lengths': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     'k4_train_march_workspace_bytes': (C.c_size_t, [C.c_int64]),
     'k4_train_march_forward': (C.c_int, [C.POINTER(TrainMarchArgs), C.c_void_p, C.c_size_t, C.c_void_p]),
     'k4_train_march_backward': (C.c_int, [C.POINTER(TrainMarchArgs), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -889,6 +889,18 @@ K4_API int k4_testing_lpips_stage(const k4_lpips* net, const float* d_img, const
                                   k4_stream_t stream);
 
 /*
+ * k4_testing_png_code_lengths: the length-limited Huffman code lengths k4_png_encode gives a histogram (package-merge,
+ * the encoder's own device routine in one CTA, as for its literal / length, distance and code-length codes), so that a
+ * test can compare them with an optimal length-limited code on histograms no frame produces.
+ *   d_freq: device int32 [n] counts, 1 <= n <= 286; a count <= 0 gets length 0.  maxbits: 1..15.
+ *   d_len: device uint8 [n], receives the lengths.  Counts the routine cannot code -- more non-zero counts than
+ *   2^maxbits, or a total of 2^31 - 1 or more -- give 0xff for every length.
+ * Arguments are checked before any CUDA call (K4_ERR_INVALID_ARG).  Caller's stream, no host sync.
+ */
+K4_API int k4_testing_png_code_lengths(const int32_t* d_freq, int32_t n, int32_t maxbits, uint8_t* d_len,
+                                       k4_stream_t stream);
+
+/*
  * PNG files of uint8 RGB frames on the device, for run_sr.py --render_test's imageio.imwrite of every frame
  * (csrc/k4_png.cu; DESIGN.md section 3.10).
  *   d_rgb: u8 [H, W, 3] contiguous (frame_u8 / render_frame_4k(out_u8=True)'s layout).

@@ -14,7 +14,7 @@ def declared_symbols():
 def test_header_declares_expected_entry_points():
     syms = declared_symbols()
     for s in ('k4_scene_create', 'k4_scene_destroy', 'k4_render_rays', 'k4_render_workspace_bytes',
-              'k4_make_rays', 'k4_abi_version', 'k4_status_string'):
+              'k4_make_rays', 'k4_abi_version', 'k4_status_string', 'k4_png_encode', 'k4_testing_png_code_lengths'):
         assert s in syms
 
 
@@ -219,6 +219,19 @@ def test_testing_skip_field_validates_arguments_without_a_gpu():
     cd[:] = [7, 7, 7]
     assert lib.k4_testing_skip_field(C.addressof(scene), C.addressof(buf), 64, cd) == -2
     assert list(cd) == [0, 0, 0]
+
+
+def test_testing_png_code_lengths_validates_arguments_without_a_gpu():
+    """k4_testing_png_code_lengths (the PNG encoder's code lengths of a histogram, for the GPU tests): a NULL buffer,
+    n outside 1..286 or maxbits outside 1..15 is K4_ERR_INVALID_ARG before any CUDA call."""
+    from k4nerf import _lib
+    C = ctypes
+    lib = _lib.lib
+    f = C.addressof(C.create_string_buffer(4 * 300))
+    ln = C.addressof(C.create_string_buffer(300))
+    for args in ((None, 19, 7, ln), (f, 19, 7, None), (f, 0, 7, ln), (f, -1, 7, ln), (f, 287, 15, ln), (f, 30, 0, ln),
+                 (f, 30, 16, ln), (f, 30, -3, ln)):
+        assert lib.k4_testing_png_code_lengths(*args, None) == -1, args
 
 
 def test_testing_srnet_forward_upto_validates_arguments_without_a_gpu():
