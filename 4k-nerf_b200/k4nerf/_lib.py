@@ -221,6 +221,10 @@ EXPORTS = {
     'k4_op_rgb_ssim': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.POINTER(C.c_int64),
                                  C.POINTER(C.c_int64), C.POINTER(C.c_double), C.c_int32, C.c_double, C.c_double, C.c_void_p,
                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    'k4_op_resize_quarter': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.POINTER(C.c_int64), C.c_void_p, C.c_void_p]),
+    'k4_op_mse_f32_workspace_bytes': (C.c_size_t, [C.c_int64, C.c_int64]),
+    'k4_op_mse_f32': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                C.POINTER(C.c_int32), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     'k4_lpips_create': (C.c_int, [C.c_int32, C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
     'k4_lpips_destroy': (C.c_int, [C.c_void_p]),
     'k4_lpips_workspace_bytes': (C.c_size_t, [C.c_void_p, C.c_int64, C.c_int64]),

@@ -250,6 +250,71 @@ def render_test_4k(model, net_sr, render_poses, HW, Ks, ndc, render_kwargs, gt_i
 
 
 @torch.no_grad()
+def render_val_4k(model, net_sr, poses, HW, Ks, ndc, render_kwargs, gt_imgs, srgt, load_sr, savedir=None, global_step=0,
+                  sel_b=0, test_tile=510, dump_images=False, eval_ssim=False, eval_lpips_alex=False, eval_lpips_vgg=False,
+                  lpips_weights=None, flip_x=None, flip_y=None):
+    """The joint stage's validation block of run_sr.py (run_sr.py:1088-1146) with every SR frame scored and written on
+    the device.  Each view is one :func:`render_frame_4k` pass; its LR results are :func:`render_viewpoints_sr`'s on the
+    same inputs, bit for bit, scored against ``gt_imgs`` and dumped (``dump_images``) as there.  The clamped SR frame
+    stays on the device and is scored against ``srgt[i]`` (the block's ``rgb_srgt_val``: numpy arrays or CUDA tensors,
+    uploaded once in their own layout):
+
+    * ``sr_psnr = -10. * np.log10(utils.rgb_mse(sr, gt))``: numpy's float32 value bit for bit;
+    * ``sr_ssim = utils.rgb_ssim(sr, gt, max_val=1)``;
+    * ``sr_lpips = utils.rgb_lpips`` (VGG, ``lpips_weights`` as its ``weights``) of ``utils.resize_quarter`` of both
+      frames when ``load_sr == 1`` (cv2's ``fx = fy = 1/4``), of the frames themselves otherwise.
+
+    With ``savedir``, ``test_<global_step>.png`` (``to8b`` of the LR frame) and ``testsr_<global_step>_<sel_b>.png`` (of
+    the SR frame) are written from the device for every view, as the reference overwrites them.  The reference's three
+    ``Testing ... (sr)`` lines are printed per view after the LR report.  Returns ``render_viewpoints_sr``'s
+    ``(rgbs, depths, bgmaps, psnrs, viewdirs_all, rgb_features)`` followed by the per-view lists ``sr_psnrs``,
+    ``sr_ssims`` and ``sr_lpips``; choosing and saving the checkpoint stays with the caller."""
+    import os
+    from .utils import frame_u8_cuda, resize_quarter, rgb_mse, write_png
+    assert len(poses) == len(HW) and len(HW) == len(Ks) and len(srgt) >= len(poses)
+    flip_x = render_kwargs.get('flip_x', False) if flip_x is None else flip_x
+    flip_y = render_kwargs.get('flip_y', False) if flip_y is None else flip_y
+    dev = next(model.parameters()).device
+    srgt = torch.as_tensor(srgt).to(dev)
+    rgbs, rgb_features, depths, bgmaps, psnrs, ssims, viewdirs_all = [], [], [], [], [], [], []
+    lpips_alex, lpips_vgg, sr_psnrs, sr_ssims, sr_lpips = [], [], [], [], []
+    for i, c2w in enumerate(poses):
+        H, W = int(HW[i][0]), int(HW[i][1])
+        sr, lr, viewdirs = _render_frame_4k(model, net_sr, H, W, Ks[i], c2w, ndc, render_kwargs, test_tile, False,
+                                            flip_x, flip_y)
+        rgb_f = lr['rgb_marched'].view(H, W, 3)
+        rgb_d = rgb_f.clamp(0, 1)
+        rgb = rgb_d.cpu().numpy()
+        rgbs.append(rgb)
+        rgb_features.append(rgb_f.cpu().numpy())
+        depths.append(lr['depth'].view(H, W, 1).cpu().numpy())
+        bgmaps.append(lr['alphainv_last'].view(H, W, 1).cpu().numpy())
+        viewdirs_all.append(viewdirs)
+        if gt_imgs is not None:
+            psnrs.append(-10. * np.log10(np.mean(np.square(rgb - gt_imgs[i]))))
+            _score(rgb_d, gt_imgs[i], eval_ssim, eval_lpips_alex, eval_lpips_vgg, ssims, lpips_alex, lpips_vgg)
+        if savedir is not None and dump_images:
+            write_png(os.path.join(savedir, 'e{}_{:03d}.png'.format(global_step, i)), frame_u8_cuda(rgb_f))
+        sr_hwc, gt = sr.permute(1, 2, 0), srgt[i]
+        sr_psnrs.append(-10. * np.log10(rgb_mse(sr_hwc, gt)))
+        sr_ssims.append(rgb_ssim(sr_hwc, gt, max_val=1))
+        if load_sr == 1:
+            sr_lpips.append(rgb_lpips(resize_quarter(sr_hwc), resize_quarter(gt), 'vgg', weights=lpips_weights))
+        else:
+            sr_lpips.append(rgb_lpips(sr_hwc, gt, 'vgg', weights=lpips_weights))
+        if savedir is not None:
+            write_png(os.path.join(savedir, f'test_{global_step}.png'), frame_u8_cuda(rgb_f))
+            write_png(os.path.join(savedir, f'testsr_{global_step}_{sel_b}.png'), frame_u8_cuda(sr_hwc))
+    _report(psnrs, ssims, lpips_vgg, lpips_alex)
+    for p, s, l in zip(sr_psnrs, sr_ssims, sr_lpips):
+        print('Testing psnr', p, '(sr)')
+        print('Testing ssim', s, '(sr)')
+        print('Testing lpips', l, '(sr)')
+    return (np.array(rgbs), np.array(depths), np.array(bgmaps), psnrs, viewdirs_all, np.array(rgb_features),
+            sr_psnrs, sr_ssims, sr_lpips)
+
+
+@torch.no_grad()
 def render_video_4k(model, net_sr, render_poses, HW, Ks, ndc, render_kwargs, render_factor=0, render_video_flipy=False,
                     render_video_rot90=0, test_tile=510, flip_x=None, flip_y=None, on_frame=None):
     """The three videos of run_sr.py --render_video (run_sr.py:1399-1463) as the uint8 arrays it hands to

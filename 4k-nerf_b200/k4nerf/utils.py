@@ -100,6 +100,136 @@ def rgb_ssim(img0, img1, max_val, filter_size=11, filter_sigma=1.5, k1=0.01, k2=
 
 
 # ------------------------------------------------------------------------------------------------
+# The joint stage's validation (run_sr.py:1131-1138): numpy's MSE and cv2's quarter-size resize
+# ------------------------------------------------------------------------------------------------
+def numpy_visit_order(shape, strides_a, strides_b):
+    """The axes of ``a - b`` (``[H, W, 3]`` operands with these element strides) from the outermost to the innermost
+    in the order numpy visits the difference's elements: numpy allocates the difference in 'K' order
+    (``npyiter_find_best_axis_ordering``: a stable insertion sort from the innermost axis by stride, where an axis
+    moves inward only if every operand with non-zero strides on both axes agrees, C order otherwise), and the mean
+    then reduces it in its memory order.  A size-1 axis has stride 0 there."""
+    nd = len(shape)
+    st = [[0 if shape[ax] == 1 else abs(int(s[ax])) for s in (strides_a, strides_b)] for ax in range(nd)]
+    perm = list(range(nd))                        # iterator axes, innermost first: axis j is array axis nd - 1 - j
+    for i0 in range(1, nd):
+        j0, ipos = perm[i0], i0
+        s0 = st[nd - 1 - j0]
+        for i1 in range(i0 - 1, -1, -1):
+            s1 = st[nd - 1 - perm[i1]]
+            ambig, swap = True, False
+            for op in range(2):
+                if s0[op] != 0 and s1[op] != 0:
+                    if s1[op] <= s0[op]:
+                        swap = False
+                    elif ambig:
+                        swap = True
+                    ambig = False
+            if not ambig:
+                if swap:
+                    ipos = i1
+                else:
+                    break
+        if ipos != i0:
+            perm[ipos + 1:i0 + 1] = perm[ipos:i0]
+            perm[ipos] = j0
+    return [nd - 1 - j for j in reversed(perm)]
+
+
+def _cuda_rgb_pair(a, b, what):
+    if not (_is_cuda(a) and _is_cuda(b) and a.device == b.device):
+        raise RuntimeError(f'{what}: both images must be CUDA tensors on one device, or both numpy arrays')
+    if a.dtype != torch.float32 or b.dtype != torch.float32:
+        raise TypeError(f'{what}: float32 images expected, got {a.dtype} and {b.dtype}')
+    if a.ndim != 3 or a.shape[-1] != 3 or a.shape != b.shape:
+        raise ValueError(f'{what}: two [H, W, 3] images of one shape expected, got {tuple(a.shape)} and {tuple(b.shape)}')
+    return a.detach(), b.detach()
+
+
+def rgb_mse(a, b):
+    """``np.mean(np.square(a - b))`` of two float32 ``[H, W, 3]`` images (run_sr.py:1132), as ``np.float32``; the PSNR
+    is ``-10. * np.log10(rgb_mse(a, b))`` (float32, as the reference's ``sr_psnr``).
+
+    CUDA tensors (both on one device, any strides, e.g. ``sr.permute(1, 2, 0)`` of a ``[3, H, W]`` frame) are scored
+    by ``k4_op_mse_f32`` with numpy's result bit for bit: the differences and squares in float32, numpy's pairwise sum
+    over the elements in the order numpy would visit arrays of those strides (:func:`numpy_visit_order`), and numpy's
+    division; one 4-byte read.  Numpy arrays and CPU tensors are numpy's own expression."""
+    if _is_cuda(a) or _is_cuda(b):
+        import ctypes as C
+        from . import _lib
+        a, b = _cuda_rgb_pair(a, b, 'rgb_mse')
+        H, W = a.shape[0], a.shape[1]
+        dev = a.device
+        with torch.cuda.device(dev):
+            ws = torch.empty(max(_lib.lib.k4_op_mse_f32_workspace_bytes(H, W), 4), dtype=torch.uint8, device=dev)
+            out = torch.empty((), dtype=torch.float32, device=dev)
+            order = (C.c_int32 * 3)(*numpy_visit_order(a.shape, a.stride(), b.stride()))
+            _cuda_call('k4_op_mse_f32', C.c_void_p(a.data_ptr()), C.c_void_p(b.data_ptr()), H, W, _strides3(a), _strides3(b),
+                       order, C.c_void_p(out.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(),
+                       C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+        return np.float32(out.item())
+    return np.mean(np.square(np.asarray(a) - np.asarray(b)))
+
+
+def resize_quarter_size(H, W):
+    """cv2's ``dsize`` for ``fx = fy = 1/4``: ``(cvRound(H / 4), cvRound(W / 4))``, halves rounded to even."""
+    return int(np.rint(H * 0.25)), int(np.rint(W * 0.25))
+
+
+def _resize_quarter_axis(n, d, clamp_last):
+    """Source pairs and weights of the ``d`` outputs along an axis of ``n`` pixels (see :func:`resize_quarter`)."""
+    k = np.arange(d)
+    inside = 4 * k + 3 <= n
+    i0 = np.where(inside, 4 * k + 1, n - 1 if clamp_last else n - 2)
+    i1 = np.where(inside, 4 * k + 2, n - 1)
+    t = np.where(inside, 0.5, 0.0 if clamp_last else 1.0).astype(np.float32)
+    return i0, i1, t
+
+
+def _lerp_f32(a, b, t):
+    """``a + (b - a) t`` in float32, one rounding per operation; ``t == 0`` is ``a`` itself."""
+    return np.where(t == 0, a, (a + (b - a) * t).astype(np.float32))
+
+
+def _resize_quarter_np(x):
+    x = np.asarray(x)
+    H, W = x.shape[0], x.shape[1]
+    h, w = resize_quarter_size(H, W)
+    rows_first = H == 3 or W == 3
+    y0, y1, ty = _resize_quarter_axis(H, h, rows_first)
+    x0, x1, tx = _resize_quarter_axis(W, w, rows_first)
+    ty, tx = ty[:, None, None], tx[None, :, None]
+    g = lambda ys, xs: x[ys][:, xs]
+    if rows_first:
+        return _lerp_f32(_lerp_f32(g(y0, x0), g(y1, x0), ty), _lerp_f32(g(y0, x1), g(y1, x1), ty), tx)
+    return _lerp_f32(_lerp_f32(g(y0, x0), g(y0, x1), tx), _lerp_f32(g(y1, x0), g(y1, x1), tx), ty)
+
+
+def resize_quarter(x):
+    """``cv2.resize(x, None, fx=1/4, fy=1/4)`` (INTER_LINEAR) of a float32 ``[H, W, 3]`` image, bit for bit with cv2
+    4.13's IPP build: the frames run_sr.py:1136 scores LPIPS on when ``load_sr == 1``.  The output is ``[h, w, 3]``
+    (:func:`resize_quarter_size`; H and W at least 3).  Along an axis of n pixels output k is ``a + (b - a) t`` of
+    pixels 4k+1 and 4k+2 with t = 0.5, or of pixels n-2 and n-1 with t = 1 when 4k + 3 > n; columns first, then rows.
+    With H or W equal to 3 cv2 goes rows first and reads pixel n-1 alone past the edge.
+
+    CUDA tensors (any strides, e.g. ``sr.permute(1, 2, 0)``) run on the GPU (``k4_op_resize_quarter``) and give a
+    contiguous CUDA tensor; numpy arrays and CPU tensors take the numpy restatement and give a numpy array."""
+    if not (x.ndim == 3 and x.shape[-1] == 3 and x.dtype in (np.float32, torch.float32)):
+        raise ValueError(f'resize_quarter: a float32 [H, W, 3] image expected, got {x.dtype} {tuple(x.shape)}')
+    H, W = x.shape[0], x.shape[1]
+    if H < 3 or W < 3:
+        raise ValueError(f'resize_quarter: {H} x {W} has no pixels at a quarter of its size (cv2 rejects it too)')
+    if not _is_cuda(x):
+        return _resize_quarter_np(x)
+    import ctypes as C
+    x = x.detach()
+    out = torch.empty((*resize_quarter_size(H, W), 3), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        _cuda_call('k4_op_resize_quarter', C.c_void_p(x.data_ptr()), H, W, _strides3(x), C.c_void_p(out.data_ptr()),
+                   C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream))
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
 # LPIPS (lib/utils.py:137-149)
 # ------------------------------------------------------------------------------------------------
 _LPIPS_NETS = {'vgg': 0, 'alex': 1}                                 # K4_LPIPS_VGG / K4_LPIPS_ALEX

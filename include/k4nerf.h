@@ -493,6 +493,39 @@ K4_API int k4_op_rgb_ssim(const void* d_img0, const void* d_img1, int32_t dtype,
                           double* d_map, double* d_mean, void* d_workspace, size_t workspace_bytes, k4_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * The joint stage's validation scores (csrc/k4_val.cu; DESIGN.md section 3.11).
+ *
+ * k4_op_resize_quarter replaces cv2.resize(img, None, fx=1/4, fy=1/4) (INTER_LINEAR, run_sr.py:1136) of an fp32
+ * H x W x 3 image, bit for bit with cv2 4.13's IPP build.  d_src: element (y, x, c) at y * strides[0] + x * strides[1] +
+ * c * strides[2] (HOST array of element strides, each >= 0).  d_dst: fp32 [h, w, 3] contiguous, h = cvRound(H / 4),
+ * w = cvRound(W / 4) (halves round to even).  Per axis of n pixels, output k interpolates pixels 4k+1 and 4k+2 with
+ * t = 0.5, or, when 4k + 3 > n, pixels n-2 and n-1 with t = 1, as a + (b - a) t with one rounding per operation; along
+ * columns first, then rows.  With H or W equal to 3, rows first, and a pair past the edge reads pixel n-1 alone.
+ * A NULL or misaligned pointer, a negative stride, or H or W outside 3 .. 65535: K4_ERR_INVALID_ARG, before any CUDA
+ * call.  Caller's stream, no host sync, no allocation.
+ *
+ * k4_op_mse_f32 replaces np.mean(np.square(a - b)) of two float32 H x W x 3 arrays (run_sr.py:1132), bit for bit:
+ * d = a - b and d * d in fp32, their sum in numpy's pairwise order (loops_utils.h's pairwise_sum over all 3 H W values),
+ * added to 0, and *d_mse = float32(float64(sum) / (3 H W)) as numpy's mean computes it.  d_a, d_b and their strides as
+ * k4_op_resize_quarter's source.  order: HOST int32[3], the axes (0 = y, 1 = x, 2 = c) from the outermost to the
+ * innermost in the order numpy visits the difference's elements (its memory order: {0, 1, 2} for C-contiguous
+ * operands, {2, 0, 1} when both are [3, H, W] planes viewed as [H, W, 3]).  The workspace holds
+ * k4_op_mse_f32_workspace_bytes(H, W) bytes, 4-byte aligned (0: an invalid shape).  The sum's tree depends on 3 H W
+ * only and is evaluated without atomics, so the result is bitwise reproducible.  Caller's stream, no host sync.
+ * A NULL or misaligned pointer, a negative stride, H or W outside 1 .. 65535, or an order that is not a permutation of
+ * {0, 1, 2}: K4_ERR_INVALID_ARG; a workspace smaller than the size: K4_ERR_WORKSPACE; both before any CUDA call.
+ */
+/* Replaces: cv2.resize(rgb, dsize=None, fx=1/4, fy=1/4) (run_sr.py:1136). */
+K4_API int k4_op_resize_quarter(const float* d_src, int64_t H, int64_t W, const int64_t strides[3], float* d_dst,
+                                k4_stream_t stream);
+/* Replaces: np.mean(np.square(rgb_srsave - rgb_srgt_val[idx])) (run_sr.py:1132) -- the workspace of k4_op_mse_f32. */
+K4_API size_t k4_op_mse_f32_workspace_bytes(int64_t H, int64_t W);
+/* Replaces: np.mean(np.square(rgb_srsave - rgb_srgt_val[idx])) (run_sr.py:1132). */
+K4_API int k4_op_mse_f32(const float* d_a, const float* d_b, int64_t H, int64_t W, const int64_t strides_a[3],
+                         const int64_t strides_b[3], const int32_t order[3], float* d_mse, void* d_workspace,
+                         size_t workspace_bytes, k4_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * LPIPS (csrc/k4_lpips.cu).
  *
  * Replaces: utils.rgb_lpips (lib/utils.py:137-149), lpips.LPIPS(net='vgg' | 'alex', version='0.1') called with
